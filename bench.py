@@ -11,8 +11,13 @@ ranks) in the PARITY-BACKED mode ("mixed": fp32-faithful 3-pass forward + single
 checked against the CPU oracle at 1e-3 inside this run, key `parity_b64`); `e2e` = the same through the public module API
 with pinned host inputs (H2D copies + D2H loss read in the timed region); `modes` = the other precision modes on the same
 workload ("half" single-pass throughput mode, "fp32x3" 3-pass forward AND backward); `roofline` = tensor-core fraction of the
-tcgen05 conv kernel family measured live with CUDA events; `cpu_baseline` = the CPU oracle timed on this box's host cores;
-`cudnn_same_gpu` = the reference algorithm as PyTorch/cuDNN ops on this same GPU (TF32, channels_last, AMP variants).
+wgmma conv kernel family measured live with CUDA events; `cpu_baseline` = the CPU oracle timed on this box's host cores;
+`cudnn_same_gpu` = the reference algorithm as PyTorch/cuDNN ops on this same GPU (TF32, channels_last, AMP variants); `gpu` =
+the card's name and power limit, read in the same run.
+
+--dump-outputs DIR writes what the timed path computed in its last timed step as DIR/<name>.npy (float32): the 8 losses, a
+fixed seeded sample of the head output and of the parameter gradients (train configs), or rot / t (--config pnp).  Inputs and
+weights are seeded, so two builds run with the same arguments can be compared output for output.
 """
 from __future__ import annotations
 
@@ -60,9 +65,43 @@ def load_peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         d = json.load(open(p))
-        return dict(bf16_sustained=d.get("bf16_tflops_sustained", 1453.0), bf16_burst=d.get("bf16_tflops", 1718.7),
-                    hbm=d.get("hbm_gbs", 6571.6), source="measured (MEASURED_PEAKS.json)")
-    return dict(bf16_sustained=1400.0, bf16_burst=1590.0, hbm=6650.0, source="fallback (B200_PROFILING.md)")
+        return dict(bf16_sustained=d.get("bf16_tflops_sustained", 989.0), bf16_burst=d.get("bf16_tflops", 989.0),
+                    hbm=d.get("hbm_gbs", 3350.0), source="measured (MEASURED_PEAKS.json)")
+    # NVIDIA H100 SXM data sheet (700 W card): dense BF16 / FP16 989 TFLOP/s, HBM3 3.35 TB/s -- never reached, a bound
+    return dict(bf16_sustained=989.0, bf16_burst=989.0, hbm=3350.0, source="H100 SXM data sheet (dense, 700 W)")
+
+
+def smi_id(index: int) -> str:
+    """nvidia-smi's id of CUDA device `index`: its PCI bus id.  nvidia-smi numbers cards by physical index, which differs from
+    the CUDA index whenever CUDA_VISIBLE_DEVICES selects or reorders cards."""
+    p = torch.cuda.get_device_properties(index)
+    return f"{p.pci_domain_id:08X}:{p.pci_bus_id:02X}:{p.pci_device_id:02X}.0"
+
+
+def gpu_info(index: int) -> dict:
+    """Name and power limit of the card the numbers were measured on (a power-limited card runs lower clocks)."""
+    info = {"name": torch.cuda.get_device_name(index), "pci_bus_id": smi_id(index), "power_limit_w": None}
+    try:
+        r = subprocess.run(["nvidia-smi", f"--id={info['pci_bus_id']}", "--query-gpu=power.limit", "--format=csv,noheader,nounits"],
+                           capture_output=True, text=True, timeout=20)
+        info["power_limit_w"] = float(r.stdout.strip().splitlines()[0])
+    except Exception:
+        pass
+    return info
+
+
+def dump_outputs(out_dir: str, arrays: dict, sample: int = 1 << 21):
+    """DIR/<name>.npy in float32; arrays longer than `sample` are reduced to a fixed seeded sample of their flat entries
+    (same indices in every run for the same length), so the files stay well under 64 MB in all."""
+    import numpy as np
+
+    os.makedirs(out_dir, exist_ok=True)
+    for name, t in arrays.items():
+        a = t.detach().float().cpu().reshape(-1).numpy()
+        if a.size > sample:
+            idx = np.sort(np.random.default_rng(0).choice(a.size, size=sample, replace=False))
+            a = a[idx]
+        np.save(os.path.join(out_dir, name + ".npy"), a.astype(np.float32))
 
 
 class ClockSampler:
@@ -76,7 +115,7 @@ class ClockSampler:
     def start(self):
         try:
             self.proc = subprocess.Popen(
-                ["nvidia-smi", f"--id={self.index}",
+                ["nvidia-smi", f"--id={smi_id(self.index)}",
                  "--query-gpu=clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
                  "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
                  "clocks_event_reasons.sw_power_cap", "--format=csv,noheader,nounits", "-lms", "100"],
@@ -224,23 +263,27 @@ def run_ours(args):
             ms = float(t)
         assert torch.isfinite(losses).all(), "non-finite losses"
         step_losses, step_logits = last["losses"].clone(), last["logits"].clone()  # outputs of the last TIMED step
+        step_grad = eng.flat_grad.clone() if (with_clocks and args.dump_outputs) else None
         if graphed is not None:  # launches inside a replayed graph are not seen by the library's host-side counter
             l1 = launch_count()
             eager_step()
             launches = launch_count() - l1
             torch.cuda.synchronize()
         return dict(model=model, eng=eng, ms=ms, launches=launches, clocks=clocks, batch=batch, losses=step_losses,
-                    logits=step_logits, graphed=graphed is not None, precision=precision)
+                    logits=step_logits, grad=step_grad, graphed=graphed is not None, precision=precision)
 
     main = one_mode(HEADLINE_MODE, args.steps, args.warmup, with_clocks=True)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, {"losses": main["losses"], "head_logits": main["logits"], "param_grads": main["grad"]})
+    main["grad"] = None
     ms = main["ms"]
     value = world * B / (ms / 1e3)
     mode_desc = {
-        "mixed": "fp32-faithful forward (hi/lo fp16 planes = 22-bit operands, 3 tcgen05 passes, fp32 accumulate) + single-pass "
+        "mixed": "fp32-faithful forward (hi/lo fp16 planes = 22-bit operands, 3 wgmma passes, fp32 accumulate) + single-pass "
                  "fp16 backward (loss scale 1024); forward outputs / losses checked at 1e-3 against the CPU oracle at B=64 "
                  "(parity_b64), gradients at the fp32x3 bound (tests/test_parity_b64_gpu.py)",
-        "fp32x3": "hi/lo fp16 planes (22-bit operands), 3 tcgen05 passes in forward and backward",
-        "half": "single fp16 plane, one tcgen05 pass (TF32-class operands; NOT inside the 1e-3 parity bound)",
+        "fp32x3": "hi/lo fp16 planes (22-bit operands), 3 wgmma passes in forward and backward",
+        "half": "single fp16 plane, one wgmma pass (TF32-class operands; NOT inside the 1e-3 parity bound)",
     }
 
     out = {
@@ -255,10 +298,11 @@ def run_ours(args):
                                 "crop, device-resident table), ResNet-34 GDR-Net full fwd+bwd incl. all 8 losses, batch 32/GPU, 256x256 synthetic crops"),
                    "precision_mode": HEADLINE_MODE + ": " + mode_desc[HEADLINE_MODE],
                    "global_batch": world * B, "parallelism": f"dp{world}",
-                   "l2": "activations per step (>2 GB) exceed the 126 MB L2; no explicit flush",
+                   "l2": "activations per step (>2 GB) exceed the 50 MB L2; no explicit flush",
                    "launch": "whole step (incl. the NCCL all-reduces at N>1) replayed as one CUDA graph" if main["graphed"] else "eager (one ctypes call per kernel)",
+                   "reductions": "ordered BatchNorm statistics / backward sums (reproducible run to run)" if main["eng"].deterministic else "fp32 atomics (GDRN_DETERMINISTIC=0; not reproducible)",
                    "grad_exchange": "bucketed NCCL all-reduce (AVG) of the flat 140 MB fp32 gradient buffer on a side stream, overlapped with backward, captured in the step graph" if world > 1 else "none"},
-        "clocks": main["clocks"], "gpu_launches": int(main["launches"]),
+        "clocks": main["clocks"], "gpu": gpu_info(local), "gpu_launches": int(main["launches"]),
     }
 
     if args.quick:
@@ -318,7 +362,7 @@ def run_ours(args):
             loss_ev[i_last & 1].synchronize()
             read_back.append(float(loss_host[i_last & 1]))
 
-        n_e2e = max(3, args.steps)
+        n_e2e = args.steps
         cur = upload()
         # >= 8 untimed steps: the first one captures the forward / backward graphs, the next few let the caching allocator reach
         # its steady state (the prefetched input tensors are held by record_stream for a step, so early steps still cudaMalloc)
@@ -357,7 +401,7 @@ def run_ours(args):
                              "on a copy stream) and every step's loss is read back to the host (4-byte async D2H, consumed one step later)"}
 
     if rank == 0:
-        # ---- roofline of the dominant kernel family (tcgen05 implicit-GEMM conv: fwd + dgrad + wgrad), measured live
+        # ---- roofline of the dominant kernel family (wgmma implicit-GEMM conv: fwd + dgrad + wgrad), measured live
         out["roofline"] = roofline_live(main, peaks)
         if world == 1:
             main_small = dict(losses=main["losses"].cpu(), logits=main["logits"].cpu(), precision=main["precision"])
@@ -369,7 +413,7 @@ def run_ours(args):
                     out["modes"][prec] = {"value": round(B / (ms / 1e3), 1), "unit": "crops/s", "ms_per_step": round(ms, 3), "headline": True}
                     continue
                 try:
-                    r = one_mode(prec, max(5, args.steps // 2), 3, with_clocks=False)
+                    r = one_mode(prec, args.steps, args.warmup, with_clocks=False)
                     out["modes"][prec] = {"value": round(B / (r["ms"] / 1e3), 1), "unit": "crops/s", "ms_per_step": round(r["ms"], 3),
                                           "what": mode_desc[prec]}
                     del r
@@ -377,14 +421,14 @@ def run_ours(args):
                 except Exception as e:  # pragma: no cover
                     out["modes"][prec] = {"error": str(e)[:200]}
             try:
-                out["inference"] = inference_bench(B, dev, peaks)
+                out["inference"] = inference_bench(B, dev, peaks, steps=args.steps, warm=args.warmup)
             except Exception as e:  # pragma: no cover
                 out["inference"] = {"error": str(e)[:300]}
             cb, parity = cpu_baseline(sample_batch=args.cpu_batch, iters=args.cpu_iters, check=main_small)
             out["cpu_baseline"] = cb
             out["parity_b64"] = parity
             try:
-                out["cudnn_same_gpu"] = cudnn_same_gpu(B, dev)
+                out["cudnn_same_gpu"] = cudnn_same_gpu(B, dev, steps=args.steps, warm=args.warmup)
             except Exception as e:  # pragma: no cover
                 out["cudnn_same_gpu"] = {"error": str(e)[:300]}
         print(json.dumps(out), flush=True)
@@ -392,7 +436,7 @@ def run_ours(args):
 
 
 def roofline_live(main, peaks):
-    """Time every tcgen05 GEMM launch of one step with CUDA events (on the launching stream) and divide the
+    """Time every wgmma GEMM launch of one step with CUDA events (on the launching stream) and divide the
     algorithmic FLOPs (2*M*N*K of the convolution / linear it implements) by the summed durations."""
     from gdr_net_b200 import ops
 
@@ -415,7 +459,7 @@ def roofline_live(main, peaks):
             r = fn(*a, **k)
             e1.record()
             variant = _C.load().gdrn_last_gemm_variant() if name in ("conv_fwd", "gemm_fwd", "conv_dgrad_s2") else 0
-            passes = a[1].nsplit if name in ("conv_wgrad", "gemm_wgrad") else a[0].nsplit  # tcgen05 passes per algorithmic MAC
+            passes = a[1].nsplit if name in ("conv_wgrad", "gemm_wgrad") else a[0].nsplit  # wgmma passes per algorithmic MAC
             records.append((name, flops_of(*a, **k), e0, e1, variant, passes))
             return r
 
@@ -479,8 +523,7 @@ def roofline_live(main, peaks):
             fwd_gemm_ms += ms_
             fwd_mma += fl * passes
         if variant:
-            kname = "gemm_fwd2_kernel" if variant >= 10000 else "gemm_fwd_kernel"  # fwd2 = cta_group::2 pair tiles
-            key = f"gdrn::{kname}<{(variant % 10000) // 10}, {variant % 10}>"
+            key = f"gdrn::gemm_fwd_kernel<{variant // 10}, {variant % 10}>"
             d = inst.setdefault(key, [0.0, 0.0, 0, 0.0])
             d[0] += fl
             d[1] += ms_
@@ -494,23 +537,17 @@ def roofline_live(main, peaks):
     dom_mma = dom[1][3] / (dom[1][1] * 1e-3) / 1e12
     # the timed region of this benchmark is a fraction of a second at full boost clocks: the comparator is the BURST peak
     peak = peaks["bf16_burst"]
-    prof = {}
-    ppath = os.path.join(ROOT, "profiles", "ncu_kernel_facts.json")  # written from committed ncu captures, keyed by kernel name
-    if os.path.exists(ppath):
-        prof = json.load(open(ppath)).get(dom[0], {})
     tf = lambda fl, ms_: round(fl / (ms_ * 1e-3) / 1e12, 1) if ms_ > 0 else None  # noqa: E731
     return {
-        "bound": "tensor", "kernel": dom[0] + " (tcgen05 implicit-GEMM conv forward / dgrad" + (", cta_group::2 pair tiles)" if "fwd2" in dom[0] else ")"),
+        "bound": "tensor", "kernel": dom[0] + " (wgmma implicit-GEMM conv forward / dgrad)",
         "achieved": round(dom_tflops, 1), "peak": peak, "unit": "TFLOP/s", "frac": round(dom_tflops / peak, 4),
-        "peak_source": "bf16_tflops (burst; fp16 and bf16 tcgen05 rates are equal) of " + peaks["source"]
-                       + ": the timed region is < 1 s at full boost clocks",
+        "peak_source": "bf16_tflops (fp16 and bf16 wgmma rates are equal) of " + peaks["source"],
         "achieved_note": "ALGORITHMIC FLOPs (2*M*N*K of the conv) / summed launch durations; the 3-pass instantiations execute "
-                         "3 tcgen05 MMAs per algorithmic MAC, `mma_tflops` is that executed rate (what the tensor pipe sees)",
+                         "3 wgmma MMAs per algorithmic MAC, `mma_tflops` is that executed rate (what the tensor pipe sees)",
         "mma_tflops": round(dom_mma, 1), "mma_frac": round(dom_mma / peak, 4),
         "launches_per_step": dom[1][2], "avg_launch_ms": round(dom[1][1] / dom[1][2], 4),
         "algorithmic_gflop_per_launch": round(dom[1][0] / dom[1][2] / 1e9, 2), "share_of_step": round(dom[1][1] / step_ms, 3),
-        "traffic": prof.get("dram_bytes_per_launch"), "traffic_note": prof.get("note", "no ncu --set full capture of this instantiation committed yet"),
-        "tensor_pipe_pct_ncu": prof.get("tensor_pipe_pct"),
+        "traffic": None, "traffic_note": "not measured",
         "gemm_family": {"achieved": tf(tot_fl, tot_ms), "frac": round(tot_fl / (tot_ms * 1e-3) / 1e12 / peak, 4),
                         "mma_tflops": tf(tot_mma, tot_ms), "mma_frac": round(tot_mma / (tot_ms * 1e-3) / 1e12 / peak, 4),
                         "share_of_step": round(tot_ms / step_ms, 3), "launches_per_step": sum(v[2] for v in fam.values()),
@@ -582,7 +619,7 @@ def run_pnp(args):
             ms = float(tt)
         # e2e: host buffers in, host results out, every step
         e0.record()
-        n_e2e = max(3, args.steps // 4)
+        n_e2e = args.steps
         for _ in range(n_e2e):
             r_, t_ = net(coor_h.to(dev, non_blocking=True), reg_h.to(dev, non_blocking=True), ext_h.to(dev, non_blocking=True))
             r_host, t_host = r_.cpu(), t_.cpu()
@@ -598,6 +635,8 @@ def run_pnp(args):
         finish_distributed(world)
         return
     main = results["fp32x3"]
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, {"rot": main["rot"], "t": main["t"]})
     # algorithmic work (SURVEY 8d config 4): Conv / Linear MACs x 2 with the true nIn; bytes = fp32 input maps + fp32 weights
     flops = 2.0 * B * (1024 * 128 * 9 * nin + 256 * 128 * 9 * 128 + 64 * 128 * 9 * 128 + 8192 * 1024 + 1024 * 256 + 256 * 9)
     wbytes = 4.0 * sum(p.numel() for p in net.parameters())
@@ -626,11 +665,11 @@ def run_pnp(args):
         torch.cuda.synchronize()
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         e0.record()
-        for _ in range(10):
+        for _ in range(args.steps):
             O.pnp_forward(coor, reg, ext, sd_dev)
         e1.record()
         torch.cuda.synchronize()
-    ms_cudnn = e0.elapsed_time(e1) / 10
+    ms_cudnn = e0.elapsed_time(e1) / args.steps
     ms = main["ms"]
     line = {
         "metric": "crops/sec (stand-alone Patch-PnP forward, 64x64 maps, bs512 per GPU)", "value": round(world * B / ms * 1e3, 1), "unit": "crops/s",
@@ -639,8 +678,8 @@ def run_pnp(args):
         "config": {"workload": f"configs[3]: Patch-PnP isolation, [512, {nin}, 64, 64] correspondence maps (xyz{'+2D' if c_feat == 5 else ''} + 64 region "
                                "channels) + extents -> rot6d | t; NCHW fp32 inputs resident in HBM; one CUDA graph per step "
                                "(pack -> 3x(conv3x3 s2 + GN + ReLU) -> fc1 -> fc2 -> fc_r|fc_t)",
-                   "global_batch": world * B, "parallelism": f"replicas x{world}", "l2": "input maps (580 MB) exceed the 126 MB L2"},
-        "clocks": main["clocks"], "gpu_launches": int(launches),
+                   "global_batch": world * B, "parallelism": f"replicas x{world}", "l2": "input maps (580 MB) exceed the 50 MB L2"},
+        "clocks": main["clocks"], "gpu": gpu_info(local), "gpu_launches": int(launches),
         "e2e": {"value": round(world * B / main["ms_e2e"] * 1e3, 1), "unit": "crops/s", "ms_per_step": round(main["ms_e2e"], 3),
                 "h2d_bytes_per_step": int(coor_h.numel() * 4 + reg_h.numel() * 4 + ext_h.numel() * 4), "d2h_bytes_per_step": B * 9 * 4,
                 "api": "ConvPnPNet.forward(coor_feat, region, extents) with pinned host tensors in, host rot/t out, every step"},
@@ -662,7 +701,7 @@ def run_pnp(args):
     finish_distributed(world)
 
 
-def inference_bench(B, dev, peaks, steps=20, warm=5):
+def inference_bench(B, dev, peaks, steps, warm):
     """Forward-only (eval mode, the reference's inference caller gdrn_evaluator.py:568-580) through the public module API with
     inputs resident: every conv + BatchNorm (+ identity) + ReLU is ONE kernel (BatchNorm folded into the packed weights and
     the GEMM epilogue).  Reports crops/s and the forward tensor-core utilisation (north_star: >= 60 % on backbone+head fwd)."""
@@ -699,7 +738,7 @@ def inference_bench(B, dev, peaks, steps=20, warm=5):
     return res
 
 
-def cudnn_same_gpu(B, dev, steps=8, warm=4):
+def cudnn_same_gpu(B, dev, steps, warm):
     """The reference algorithm as plain PyTorch ops (cuDNN / cuBLAS / ATen library kernels) on THIS GPU -- what the reference's
     own nn.Modules dispatch to on the box (the reference package itself needs detectron2 / mmcv and cannot travel): the oracle
     restatement (pinned bit-exact to the live reference on CPU) on cuda, cudnn.benchmark = True
@@ -833,7 +872,7 @@ def run_reference(args):
         o = O.gdrn_forward(leaf, batch, train=True, do_loss=True)
         sum(o["losses"].values()).backward()
 
-    steps, warm = max(1, min(args.steps, 5)), max(1, min(args.warmup, 2))
+    steps, warm = args.steps, args.warmup
     for _ in range(warm):
         step()
     t0 = time.perf_counter()
@@ -866,13 +905,15 @@ def main():
     ap.add_argument("--nin", type=int, default=69, choices=[67, 69], help="--config pnp: Patch-PnP input channels")
     ap.add_argument("--quick", action="store_true", help="device-timed value only (for profiler runs)")
     ap.add_argument("--no-graph", dest="graph", action="store_false", help="launch every kernel from Python instead of one CUDA graph")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the outputs of the last timed step as DIR/<name>.npy (float32; large arrays as a fixed seeded sample)")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3)
     if args.impl == "reference":
         run_reference(args)
     else:
         if not torch.cuda.is_available():
-            raise SystemExit("bench.py needs a CUDA device (B200); there is no CPU fallback for the product path")
+            raise SystemExit("bench.py needs a CUDA device (H100); there is no CPU fallback for the product path")
         if args.config == "pnp":
             run_pnp(args)
         else:

@@ -8,7 +8,7 @@ checkpoints load unchanged, same `get_event_storage().put_scalars(**vis_dict)` s
 
 The `nn.Module`s below only OWN the parameters / buffers (ordinary `nn.Parameter`s, so optimizers,
 DDP and checkpointers see the usual thing).  All compute is done by `engine.Engine` through the C ABI
-of libgdrn_b200.so (hand-written sm_100a kernels); there is no PyTorch / CPU fallback path.
+of libgdrn_b200.so (hand-written sm_90a kernels); there is no PyTorch / CPU fallback path.
 """
 from __future__ import annotations
 
@@ -263,7 +263,7 @@ class GDRN(nn.Module):
                 roi_cams=None, roi_centers=None, roi_whs=None, roi_extents=None, resize_ratios=None, do_loss=False):
         cfg = self.cfg
         if not x.is_cuda:
-            raise RuntimeError("gdr_net_b200.GDRN runs on CUDA (sm_100a) only; there is no CPU fallback")
+            raise RuntimeError("gdr_net_b200.GDRN runs on CUDA (sm_90a) only; there is no CPU fallback")
         pnp_cfg = cfg.MODEL.CDPN.PNP_NET
         res = self.engine.run(
             x, roi_coord_2d=roi_coord_2d, roi_cams=roi_cams, roi_centers=roi_centers, roi_whs=roi_whs,

@@ -1,4 +1,4 @@
-"""gdr_net_b200 -- B200-native (sm_100a) implementation of the GDR-Net train/infer hot path.
+"""gdr_net_b200 -- H100-native (sm_90a) implementation of the GDR-Net train/infer hot path.
 
 Public surface mirrors the reference module `core.gdrn_modeling.models.GDRN`:
 

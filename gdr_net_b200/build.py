@@ -1,10 +1,10 @@
-"""In-tree build of libgdrn_b200.so (hand-written sm_100a CUDA behind a C ABI).
+"""In-tree build of libgdrn_b200.so (hand-written sm_90a CUDA behind a C ABI).
 
     python -m gdr_net_b200.build            # incremental
     python -m gdr_net_b200.build --force
 
-nvcc cross-compiles for sm_100a without a GPU.  Objects go to gdr_net_b200/_build/, the shared
-library to gdr_net_b200/lib/ (git-ignored, but shipped to the GPU box by gpurun).
+nvcc cross-compiles for sm_90a (H100) without a GPU.  Objects go to gdr_net_b200/_build/, the shared
+library to gdr_net_b200/lib/ (both git-ignored build products).
 """
 from __future__ import annotations
 
@@ -21,7 +21,7 @@ LIBDIR = os.path.join(HERE, "lib")
 LIB = os.path.join(LIBDIR, "libgdrn_b200.so")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC",
     "-diag-suppress", "550",
     # 16-bit storage format of the activation / weight planes: 1 = fp16 (11-bit mantissa, TF32-equivalent; default),
     # 0 = bf16.  See csrc/ptx.cuh.

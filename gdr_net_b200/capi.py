@@ -51,7 +51,7 @@ class _Lib:
             return self._dll
         if not os.path.exists(LIB_PATH):
             raise GdrnError(
-                f"{LIB_PATH} not found: build it with `python -m gdr_net_b200.build` (nvcc, sm_100a). "
+                f"{LIB_PATH} not found: build it with `python -m gdr_net_b200.build` (nvcc, sm_90a). "
                 "There is no CPU / PyTorch fallback for the hot path."
             )
         import torch  # noqa: F401  (loads libcudart first so the library shares torch's CUDA runtime)

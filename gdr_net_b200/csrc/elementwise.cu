@@ -121,8 +121,8 @@ __global__ void bn_fold_batched_kernel(const BnFoldJob* __restrict__ jobs) {
 }
 
 // ------------------------------------------------------------------------------------------------
-// BatchNorm forward.  Design notes (ncu, profiles/r1_bn_kernels.txt): the first version kept unpacked fp32 arrays live
-// across the loads (115 registers -> 2 blocks/SM -> 24 % warps active -> 29 % of DRAM peak).  Now the 16-byte loads
+// BatchNorm forward.  Design notes: keeping unpacked fp32 arrays live across the loads costs registers and with them the
+// warps that keep HBM busy (115 registers -> 2 blocks/SM).  The 16-byte loads
 // stay PACKED in registers while in flight (4 per tensor), per-channel coefficients live in shared memory, and the
 // kernels are templated on "has lo plane" / "has residual" so unused operands cost nothing.
 // ------------------------------------------------------------------------------------------------
@@ -148,7 +148,7 @@ __device__ __forceinline__ void bn_apply_loop(const bf16* __restrict__ x_hi, con
                                               const float* s_sh, long total, int cg, int relu, uint8_t* __restrict__ mask_out,
                                               bool rev = false) {
     // rev: walk the tensor from its END to its start.  The producing GEMM wrote it front to back, so for tensors larger than
-    // the 126 MB L2 the freshest ~100 MB are the tail; this kernel's own output then leaves its HEAD in L2, which is where the
+    // the 50 MB L2 the freshest ~40 MB are the tail; this kernel's own output then leaves its HEAD in L2, which is where the
     // consuming GEMM starts (total is a multiple of cg, so a thread's channel group stays fixed in both directions).
     const long stride = (long)gridDim.x * blockDim.x;
     const long first = blockIdx.x * (long)blockDim.x + threadIdx.x;
@@ -524,7 +524,7 @@ __global__ void zero_insert_kernel(const bf16* __restrict__ x_hi, const bf16* __
 //   apply : du = gamma*invstd * (g - sums0/n - xhat * sums1/n);  optional g_out = g;  dgamma = sums1, dbeta = sums0
 // ------------------------------------------------------------------------------------------------
 constexpr int kBnBwdThreads = 256;
-constexpr int kRedRows = 4;  // rows in flight per thread of the reduction pass (ncu r2: 2 rows / 296 blocks reached 58 % of HBM peak)
+constexpr int kRedRows = 4;  // rows in flight per thread of the reduction pass: more loads in flight per thread for the HBM-bound reads
 
 // masked gradient of one 8-channel group: g = (ga [+ gb]) * [y > 0]
 template <bool LO>
@@ -792,7 +792,7 @@ __global__ void __launch_bounds__(256, 4) bn_bwd_apply_kernel(
 // GroupNorm(32 groups) + ReLU, one CTA per sample, tensor [HW][C] (C = 128 => 4 channels per group)
 // ------------------------------------------------------------------------------------------------
 // stats layout: [B][G][2] (mean, rstd).  Each thread owns one 8-channel column group (= 2 GN groups when C/G = 4)
-// A sample is split over a CLUSTER of kGnCluster CTAs (one CTA per sample used 64 of the 148 SMs at B = 64): each CTA owns a
+// A sample is split over a CLUSTER of kGnCluster CTAs (one CTA per sample would use 64 of the 132 SMs at B = 64): each CTA owns a
 // contiguous quarter of the rows, the per-group partial sums are exchanged through distributed shared memory.
 constexpr int kGnCluster = 4;
 __device__ __forceinline__ unsigned gn_cluster_rank() {

@@ -1,6 +1,6 @@
-// Tile epilogue shared by the 1-CTA (gemm_fwd.cu) and the 2-CTA cta_group::2 (gemm_fwd2.cu) implicit-GEMM kernels:
-// tcgen05.ld of this warp's 32 accumulator rows -> (+ cross-term accumulator of the 3-pass mode) -> bias -> residual ->
-// activation -> 16-bit hi[/lo] and / or fp32 stores -> per-channel sum / sum of squares for the BatchNorm batch statistics.
+// Tile epilogue of the implicit-GEMM forward kernel (gemm_fwd.cu), run by each MMA warpgroup on its 64 x BLOCK_N register
+// accumulators: (+ cross-term accumulator of the 3-pass mode) -> bias -> residual -> activation -> 16-bit hi[/lo] and / or fp32
+// stores -> per-channel sum / sum of squares for the BatchNorm batch statistics.
 #pragma once
 #include "gdrn_internal.h"
 #include "gemm_params.h"
@@ -8,159 +8,115 @@
 
 namespace gdrn {
 
-// t_acc: TMEM address of the MAIN accumulator of this tile with the warp's lane quadrant already applied (the cross-term
-//        accumulator of the 3-pass mode sits NMAIN * BLOCK_N columns further);
-// row  : row of the 128-row tile owned by this thread (quadrant * 32 + lane); tr: this warp's 32x17 fp32 transpose buffer;
-// s_stats: the CTA's [2][BLOCK_N] partial BatchNorm sums; chunks [c_begin, c_end) of 32 columns are processed.
-template <int BLOCK_N, int NSPLIT, int NMAIN>
-__device__ __forceinline__ void gemm_epilogue_tile(const GemmParams& p, uint32_t t_acc, int lane, int row, int m_tile, int n_tile, int ph,
-                                                   int c_begin, int c_end, float* tr, float* s_stats) {
+// acc    : this thread's accumulator fragment (wgmma.cuh layout), BLOCK_N / 2 main values followed, in the 3-pass mode, by
+//          BLOCK_N / 2 cross-term values (scaled by the lo-plane scale);
+// row0   : row of the 128-row tile held in acc[4j + 0..1] (acc[4j + 2..3] hold row0 + 8); q = lane % 4 selects the column pair;
+// s_stats: the CTA's [2][BLOCK_N] partial BatchNorm sums.
+// Columns are written in 32-wide chunks like the output tiles: a chunk that starts at or beyond N is left untouched, inside a
+// partial chunk the columns in [N, ldc) are zero-filled.
+template <int BLOCK_N, int NSPLIT>
+__device__ __forceinline__ void gemm_epilogue_tile(const GemmParams& p, const float* acc, int lane, int row0, int m_tile, int n_tile,
+                                                   int ph, float* s_stats) {
     __nv_bfloat16* out_hi = reinterpret_cast<__nv_bfloat16*>(p.out_hi);
     __nv_bfloat16* out_lo = reinterpret_cast<__nv_bfloat16*>(p.out_lo);
-    const long mrow = (long)m_tile * 128 + row;
-    const bool row_ok = mrow < p.M;
-    const bool all_rows = (long)(m_tile + 1) * 128 <= p.M;
-    long grow = mrow;  // output row
-    if (p.nphase) {    // (n, i, j) of the dY lattice -> pixel (2i + a, 2j + b) of the 2x larger dX
-        const long j = mrow & ((1L << p.pw_log2) - 1);
-        const long t = mrow >> p.pw_log2;
-        const long i = t & ((1L << p.ph_log2) - 1);
-        const long n = t >> p.ph_log2;
-        grow = (((n << (p.ph_log2 + 1)) + 2 * i + p.ph_a[ph]) << (p.pw_log2 + 1)) + 2 * j + p.ph_b[ph];
+    const int q = lane & 3;
+    long grow[2];
+    bool row_ok[2];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+        const long mrow = (long)m_tile * 128 + row0 + 8 * h;
+        row_ok[h] = mrow < p.M;
+        grow[h] = mrow;  // output row
+        if (p.nphase) {  // (n, i, j) of the dY lattice -> pixel (2i + a, 2j + b) of the 2x larger dX
+            const long j = mrow & ((1L << p.pw_log2) - 1);
+            const long t = mrow >> p.pw_log2;
+            const long i = t & ((1L << p.ph_log2) - 1);
+            const long n = t >> p.ph_log2;
+            grow[h] = (((n << (p.ph_log2 + 1)) + 2 * i + p.ph_a[ph]) << (p.pw_log2 + 1)) + 2 * j + p.ph_b[ph];
+        }
     }
-#pragma unroll 1
-    for (int c = c_begin; c < c_end; ++c) {
-        const int col0 = n_tile * BLOCK_N + c * 32;
-        if (col0 >= p.N) continue;  // warp-uniform
-        float f[32];
-        {
-            const uint32_t t0 = t_acc + c * 32;
-            uint32_t raw[32];
-            tmem_ld_32x32(t0, raw);
-            tmem_ld_wait();
 #pragma unroll
-            for (int j = 0; j < 32; ++j) f[j] = __uint_as_float(raw[j]);
-            if (NSPLIT == 3) {
-                const int nmain = p.num_kb < NMAIN ? p.num_kb : NMAIN;
-                for (int a2 = 1; a2 <= NMAIN; ++a2) {
-                    if (a2 < NMAIN && a2 >= nmain) continue;  // partial never written (tiny K)
-                    tmem_ld_32x32(t0 + a2 * BLOCK_N, raw);
-                    tmem_ld_wait();
-                    const float sc = (a2 == NMAIN) ? kLoInvScale : 1.f;  // cross terms carry the lo-plane scale
+    for (int j = 0; j < BLOCK_N / 8; ++j) {
+        const int cl = 8 * j + 2 * q;  // column inside the tile
+        const int col = n_tile * BLOCK_N + cl;
+        if (n_tile * BLOCK_N + 32 * (j / 4) >= p.N) continue;  // warp-uniform: chunk beyond N
+        const bool ok0 = col < p.N, ok1 = col + 1 < p.N;
+        float f[2][2];
 #pragma unroll
-                    for (int j = 0; j < 32; ++j) f[j] = fmaf(__uint_as_float(raw[j]), sc, f[j]);
-                }
+        for (int h = 0; h < 2; ++h)
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+                f[h][e] = acc[4 * j + 2 * h + e];
+                if (NSPLIT == 3) f[h][e] = fmaf(acc[BLOCK_N / 2 + 4 * j + 2 * h + e], kLoInvScale, f[h][e]);
             }
-        }
-        const bool full_chunk = (col0 + 32 <= p.N);
         if (p.bias != nullptr) {
+            const float b0 = ok0 ? __ldg(p.bias + col) : 0.f, b1 = ok1 ? __ldg(p.bias + col + 1) : 0.f;
 #pragma unroll
-            for (int j = 0; j < 32; ++j)
-                if (full_chunk || col0 + j < p.N) f[j] += __ldg(p.bias + col0 + j);
+            for (int h = 0; h < 2; ++h) {
+                f[h][0] += b0;
+                f[h][1] += b1;
+            }
         }
-        if (p.res_hi != nullptr && row_ok && full_chunk) {
-            // folded eval epilogue: + residual (the block's identity / downsample branch, same [rows][ldc] planes)
-            const __nv_bfloat16* rh = reinterpret_cast<const __nv_bfloat16*>(p.res_hi) + grow * p.ldc + col0;
-            const __nv_bfloat16* rl = p.res_lo ? reinterpret_cast<const __nv_bfloat16*>(p.res_lo) + grow * p.ldc + col0 : nullptr;
+        if (p.res_hi != nullptr && ok0) {
+            // folded eval epilogue: + residual (the block's identity / downsample branch, same [rows][ldc] planes; N % 32 == 0)
 #pragma unroll
-            for (int j = 0; j < 4; ++j) {
-                const uint4 rq = __ldg(reinterpret_cast<const uint4*>(rh) + j);
-                const uint32_t w[4] = {rq.x, rq.y, rq.z, rq.w};
-#pragma unroll
-                for (int t = 0; t < 4; ++t) {
-                    float a, b;
-                    unpack_hi2(w[t], a, b);
-                    f[8 * j + 2 * t] += a;
-                    f[8 * j + 2 * t + 1] += b;
-                }
-                if (rl != nullptr) {
-                    const uint4 q2 = __ldg(reinterpret_cast<const uint4*>(rl) + j);
-                    const uint32_t w2[4] = {q2.x, q2.y, q2.z, q2.w};
-#pragma unroll
-                    for (int t = 0; t < 4; ++t) {
-                        float a, b;
-                        unpack_lo2(w2[t], a, b);
-                        f[8 * j + 2 * t] += a;
-                        f[8 * j + 2 * t + 1] += b;
-                    }
+            for (int h = 0; h < 2; ++h) {
+                if (!row_ok[h]) continue;
+                float a, b;
+                unpack_hi2(__ldg(reinterpret_cast<const uint32_t*>(reinterpret_cast<const __nv_bfloat16*>(p.res_hi) + grow[h] * p.ldc + col)), a, b);
+                f[h][0] += a;
+                f[h][1] += b;
+                if (p.res_lo != nullptr) {
+                    unpack_lo2(__ldg(reinterpret_cast<const uint32_t*>(reinterpret_cast<const __nv_bfloat16*>(p.res_lo) + grow[h] * p.ldc + col)), a, b);
+                    f[h][0] += a;
+                    f[h][1] += b;
                 }
             }
         }
-        if (p.act == 1) {
 #pragma unroll
-            for (int j = 0; j < 32; ++j) f[j] = f[j] > 0.f ? f[j] : 0.1f * f[j];
-        } else if (p.act == 2) {
+        for (int h = 0; h < 2; ++h)
 #pragma unroll
-            for (int j = 0; j < 32; ++j) f[j] = fmaxf(f[j], 0.f);
-        }
-        if (row_ok) {
-            if (p.out_f32 != nullptr) {
-                float* dst = p.out_f32 + grow * p.ldc + col0;
-                if (full_chunk) {
-#pragma unroll
-                    for (int j = 0; j < 32; j += 4)
-                        *reinterpret_cast<float4*>(dst + j) = make_float4(f[j], f[j + 1], f[j + 2], f[j + 3]);
-                } else {
-#pragma unroll
-                    for (int j = 0; j < 32; ++j)
-                        if (col0 + j < p.ldc) dst[j] = (col0 + j < p.N) ? f[j] : 0.f;
-                }
+            for (int e = 0; e < 2; ++e) {
+                if (p.act == 1) f[h][e] = f[h][e] > 0.f ? f[h][e] : 0.1f * f[h][e];
+                else if (p.act == 2) f[h][e] = fmaxf(f[h][e], 0.f);
             }
-            if (out_hi != nullptr) {
-                uint32_t hi[16], lo[16];
+        if (col < p.ldc) {  // ldc % 8 == 0: the pair (col, col + 1) is inside or outside together
 #pragma unroll
-                for (int j = 0; j < 16; ++j) {
-                    float a = f[2 * j], b = f[2 * j + 1];
-                    if (!full_chunk) {
-                        if (col0 + 2 * j >= p.N) a = 0.f;
-                        if (col0 + 2 * j + 1 >= p.N) b = 0.f;
+            for (int h = 0; h < 2; ++h) {
+                if (!row_ok[h]) continue;
+                const float a = ok0 ? f[h][0] : 0.f, b = ok1 ? f[h][1] : 0.f;
+                if (p.out_f32 != nullptr) *reinterpret_cast<float2*>(p.out_f32 + grow[h] * p.ldc + col) = make_float2(a, b);
+                if (out_hi != nullptr) {
+                    uint32_t hi, lo;
+                    if (out_lo != nullptr) {
+                        split2(a, b, hi, lo);
+                        *reinterpret_cast<uint32_t*>(out_lo + grow[h] * p.ldc + col) = lo;
+                    } else {
+                        hi = pack_hi2(a, b);
                     }
-                    // single-plane outputs skip the residual (lo) plane arithmetic: the epilogue warps run alone on
-                    // their schedulers, so every instruction here is on the critical path of the small-K layers
-                    if (out_lo != nullptr) split2(a, b, hi[j], lo[j]); else hi[j] = pack_hi2(a, b);
-                }
-                const int ncopy = full_chunk ? 4 : ((min(p.ldc, col0 + 32) - col0) / 8);
-                uint4* dh = reinterpret_cast<uint4*>(out_hi + grow * p.ldc + col0);
-#pragma unroll
-                for (int j = 0; j < 4; ++j)
-                    if (j < ncopy) dh[j] = make_uint4(hi[4 * j], hi[4 * j + 1], hi[4 * j + 2], hi[4 * j + 3]);
-                if (out_lo != nullptr) {
-                    uint4* dl = reinterpret_cast<uint4*>(out_lo + grow * p.ldc + col0);
-#pragma unroll
-                    for (int j = 0; j < 4; ++j)
-                        if (j < ncopy)
-                            dl[j] = make_uint4(lo[4 * j], lo[4 * j + 1], lo[4 * j + 2], lo[4 * j + 3]);
+                    *reinterpret_cast<uint32_t*>(out_hi + grow[h] * p.ldc + col) = hi;
                 }
             }
         }
         if (p.stats != nullptr) {
-            // per-channel sum / sum of squares over this warp's 32 rows: transpose 16 columns at a time through a
-            // padded smem tile (conflict-free), lane l then adds column (l & 15) over row half (l >> 4).
-            // (A shuffle butterfly was latency-bound: ~60 dependent shuffles per chunk.)
+            // per-channel sum / sum of squares over the warp's 16 rows: the 8 lanes sharing q hold the same two columns
+            float s1[2], s2[2];
 #pragma unroll
-            for (int h = 0; h < 2; ++h) {
-                if (all_rows) {  // warp-uniform: every row of the tile is a valid pixel (no per-element select)
+            for (int e = 0; e < 2; ++e) {
+                const float v0 = row_ok[0] ? f[0][e] : 0.f, v1 = row_ok[1] ? f[1][e] : 0.f;
+                s1[e] = v0 + v1;
+                s2[e] = fmaf(v1, v1, v0 * v0);
 #pragma unroll
-                    for (int j = 0; j < 16; ++j) tr[lane * 17 + j] = f[h * 16 + j];
-                } else {
-#pragma unroll
-                    for (int j = 0; j < 16; ++j) tr[lane * 17 + j] = row_ok ? f[h * 16 + j] : 0.f;
+                for (int off = 4; off < 32; off <<= 1) {
+                    s1[e] += __shfl_xor_sync(0xffffffffu, s1[e], off);
+                    s2[e] += __shfl_xor_sync(0xffffffffu, s2[e], off);
                 }
-                __syncwarp();
-                float s1 = 0.f, s2 = 0.f;
-                const int col = lane & 15, r0 = (lane >> 4) * 16;
+            }
+            if (lane < 4) {
 #pragma unroll
-                for (int i = 0; i < 16; ++i) {
-                    const float v = tr[(r0 + i) * 17 + col];
-                    s1 += v;
-                    s2 = fmaf(v, v, s2);
-                }
-                s1 += __shfl_xor_sync(0xffffffffu, s1, 16);
-                s2 += __shfl_xor_sync(0xffffffffu, s2, 16);
-                __syncwarp();
-                if (lane < 16) {
-                    atomicAdd(&s_stats[c * 32 + h * 16 + lane], s1);
-                    atomicAdd(&s_stats[BLOCK_N + c * 32 + h * 16 + lane], s2);
+                for (int e = 0; e < 2; ++e) {
+                    atomicAdd(&s_stats[cl + e], s1[e]);
+                    atomicAdd(&s_stats[BLOCK_N + cl + e], s2[e]);
                 }
             }
         }

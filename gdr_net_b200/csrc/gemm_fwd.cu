@@ -1,10 +1,10 @@
-// tcgen05 / TMEM / TMA implicit-GEMM forward kernel (sm_100a).
+// wgmma / TMA implicit-GEMM forward kernel (sm_90a).
 //
 // One persistent, warp-specialised kernel serves every GEMM-shaped forward op of the GDR-Net hot
 // path (reference call sites: resnet_backbone.py:69-76 convs, cdpn_rot_head_region.py:82-135,
 // conv_pnp_net.py:76-80 + fc1/fc2/fc_r/fc_t :111-157) and, with flipped weights, every dgrad:
 //
-//   D[M = pixels][N = Cout] = sum_k A[M][K] * W[N][K]          (16-bit operands, fp32 accumulate in TMEM)
+//   D[M = pixels][N = Cout] = sum_k A[M][K] * W[N][K]          (16-bit operands, fp32 accumulate in registers)
 //
 //   * A is never materialised: for a conv, each 64-wide k-block is one (tap, channel-chunk) and its
 //     128x64 A tile is ONE 4-D TMA box {64 ch, Wo, TH, TN} of the NHWC activation tensor at the
@@ -12,32 +12,32 @@
 //     Stride-2 convs read from four phase sub-lattices (one tensor map per (row, col) parity);
 //     stride-2 DGRADS run as four output-parity phases over the un-dilated dY (gdrn_conv_dgrad_s2).
 //   * W is a K-major [Cout][KH*KW*Cin] 16-bit matrix (prepared by pack kernels), 2-D TMA boxes.
-//   * Both land in shared memory in the 128-byte-swizzled K-major layout tcgen05.mma consumes.
-//   * warp 0 = TMA producer, warp 1 = MMA issuer, warp 2 = TMEM allocator, warps 4-11 = two epilogue
-//     warpgroups (tcgen05.ld -> bias/activation -> 16-bit hi[/lo] or fp32 stores, per-channel sum /
-//     sum-of-squares for BatchNorm batch statistics).  Accumulators are double-buffered in TMEM and
-//     each warpgroup drains one buffer, so two tile epilogues overlap the MMAs of the next tiles.
-//     Producer and issuer loops run warp-uniformly (operands in uniform registers), one elected lane
-//     issues the asynchronous instructions: ~33 instructions per k-block.
+//   * Both land in shared memory in the 128-byte-swizzled K-major layout wgmma consumes.
+//   * warpgroups 0 and 1 = MMA + epilogue, each owning 64 of the 128 rows of a tile (wgmma m64nNk16,
+//     accumulators in registers; the epilogue in gemm_epilogue.cuh applies bias / residual / activation,
+//     stores 16-bit hi[/lo] or fp32 and accumulates the per-channel BatchNorm statistics).  While the MMA
+//     warpgroups run a tile's epilogue the producer already fills the stages of the next tile.
+//     Warp 8 = TMA producer.  With nine warps ptxas allots at most 168 registers per thread (three warps share one SM
+//     sub-partition's register file).  Tiles are 128 wide in one pass (64 accumulator registers) and 64 wide in three
+//     passes (main + cross accumulators, 64 registers): a 128-wide 3-pass tile needs 128 accumulator registers and, with
+//     the epilogue's row / residual / output state, spills under that limit (ptxas -v: 152 bytes).
 //   * NSPLIT = 3 is the fp32-faithful mode: operands are (hi, lo) 16-bit planes and each k-step issues
 //     hi*hi + hi*lo + lo*hi (the lo*lo term, 2^-22 relative with fp16 planes, is dropped).
 #include <stdlib.h>
-
-#include <atomic>
 
 #include "gdrn_internal.h"
 #include "gemm_epilogue.cuh"
 #include "gemm_params.h"
 #include "ptx.cuh"
+#include "wgmma.cuh"
 
 namespace gdrn {
 
 constexpr int kBlockM = 128;
 constexpr int kBlockK = 64;
 constexpr int kSmemBudget = 227 * 1024;
-constexpr int kEpiWarps = 8;                    // two epilogue warpgroups, one per TMEM accumulator buffer
-constexpr int kTrBytes = kEpiWarps * 32 * 17 * 4;  // per-warp 32x16 (+1 pad) fp32 transpose buffers for the BN statistics
-constexpr int kAuxBytes = 4096 + kTrBytes;
+constexpr int kAuxBytes = 4096;  // barriers + [2][BLOCK_N] BatchNorm partial sums
+constexpr int kThreads = 288;    // two MMA warpgroups + one producer warp
 
 template <int BLOCK_N, int NSPLIT>
 struct GemmCfg {
@@ -48,177 +48,117 @@ struct GemmCfg {
     static constexpr int STAGES_RAW = (kSmemBudget - kAuxBytes - 1024) / STAGE_BYTES;
     static constexpr int STAGES = STAGES_RAW > 8 ? 8 : STAGES_RAW;
     static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + kAuxBytes + 1024;
-    // tcgen05.mma accumulates into TMEM with round-toward-zero (measured: tools/exp_accum.py), so the error of a
-    // K-long chain grows ~ (K/16) * 2^-24.  The fp32-faithful mode therefore keeps the small cross terms
-    // (hi*lo + lo*hi) in their own accumulator and spreads the hi*hi k-blocks round-robin over three more; the
-    // epilogue adds the four partials with round-to-nearest fp32 adds.
-    // (Splitting the hi*hi chain over several accumulators was measured to change nothing at these K: the 16-bit
-    // operand planes dominate the error, so one main + one cross accumulator is used and BLOCK_N can be 128.)
-    static constexpr int NMAIN = 1;
+    // 3-pass mode: the small cross terms (hi*lo + lo*hi) are kept in their own accumulator and added to the main one with a
+    // round-to-nearest fp32 fma in the epilogue.  Each k-step issues three MMAs of width BLOCK_N, each writing one WHOLE
+    // accumulator: a_hi x [w_hi; w_lo] as one 2 * BLOCK_N-wide MMA followed by a_lo x w_hi into its upper half would read
+    // a_hi once less, but an MMA that writes part of the registers of one still in flight makes ptxas serialise the whole
+    // wgmma chain (warning C7511); the three-MMA form measured 0.9 % faster per step.
     static constexpr int NACC = (NSPLIT == 3) ? 2 : 1;
-    static constexpr int TMEM_COLS = 2 * NACC * BLOCK_N;  // double-buffered accumulator set
+    static constexpr int ACC_REGS = NACC * BLOCK_N / 2;  // per thread: 64 rows x NACC * BLOCK_N columns over 128 threads
     static_assert(STAGES >= 2, "pipeline too shallow");
-    static_assert(TMEM_COLS <= 512, "TMEM overflow");
 };
 
-// Sum the 32 lanes' values column-wise: on return lane j holds sum over lanes of v[j] (31 shuffles).
-__device__ __forceinline__ float warp_transpose_reduce(float (&v)[32], int lane) {
-#pragma unroll
-    for (int off = 16; off >= 1; off >>= 1) {
-        const bool upper = (lane & off) != 0;
-#pragma unroll
-        for (int i = 0; i < off; ++i) {
-            float send = upper ? v[i] : v[i + off];
-            float keep = upper ? v[i + off] : v[i];
-            v[i] = keep + __shfl_xor_sync(0xffffffffu, send, off);
-        }
-    }
-    return v[0];
-}
-
 template <int BLOCK_N, int NSPLIT>
-__global__ void __launch_bounds__(128 + 32 * kEpiWarps, 1) gemm_fwd_kernel(const __grid_constant__ GemmParams p) {
+__global__ void __launch_bounds__(kThreads, 1) gemm_fwd_kernel(const __grid_constant__ GemmParams p) {
     using Cfg = GemmCfg<BLOCK_N, NSPLIT>;
     constexpr int NPL = Cfg::NPL;
     constexpr int STAGES = Cfg::STAGES;
 
     // 1024-byte alignment by POINTER arithmetic on the __shared__ array (not through uintptr_t): the compiler keeps the
-    // shared address space, so the epilogue's transposes / statistics compile to STS / LDS / ATOMS instead of generic
-    // ST / LD / ATOM (+ an address-space check each) -- the BN-statistics epilogue was the bottleneck of the 64-channel layers
+    // shared address space, so the epilogue's statistics compile to shared-memory atomics instead of generic ones
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
     uint8_t* aux = smem + STAGES * Cfg::STAGE_BYTES;
     uint64_t* full_bar = reinterpret_cast<uint64_t*>(aux);
     uint64_t* empty_bar = full_bar + STAGES;
-    uint64_t* tfull_bar = empty_bar + STAGES;
-    uint64_t* tempty_bar = tfull_bar + 2;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty_bar + 2);
     float* s_stats = reinterpret_cast<float*>(aux + 512);  // [2][BLOCK_N]
-    float* s_tr = reinterpret_cast<float*>(aux + 4096);    // [kEpiWarps][32][17]
 
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
+    const int wg = threadIdx.x >> 7;
     const int num_tiles = p.num_m_tiles * p.num_n_tiles;
 
-    if (warp == 0 && lane == 0) {
+    if (threadIdx.x == 0) {
         for (int pl = 0; pl < NPL; ++pl) {
             tma_prefetch_desc(&p.tmB[pl]);
             tma_prefetch_desc(&p.tmA[pl][0]);
         }
-    }
-    if (warp == 1 && lane == 0) {
         for (int s = 0; s < STAGES; ++s) {
             mbar_init(&full_bar[s], 1);
-            mbar_init(&empty_bar[s], 1);
-        }
-        for (int a = 0; a < 2; ++a) {
-            mbar_init(&tfull_bar[a], 1);
-            mbar_init(&tempty_bar[a], 4);
+            mbar_init(&empty_bar[s], 2);  // one arrival per MMA warpgroup
         }
         fence_barrier_init();
     }
-    if (warp == 2) {
-        tmem_alloc(tmem_slot, Cfg::TMEM_COLS);
-        tmem_relinquish();
-    }
     for (int i = threadIdx.x; i < 2 * BLOCK_N; i += blockDim.x) s_stats[i] = 0.f;
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
     pdl_launch_dependents();  // the next kernel of the stream may start its prologue under our tail
     pdl_wait();               // nothing above touched global memory; from here on we read what the predecessor wrote
     // persistent CTAs stride over the tile list (phase-major for the stride-2 dgrad)
-    const int my_cluster = blockIdx.x, num_clusters = gridDim.x;
+    const int my_cta = blockIdx.x, num_ctas = gridDim.x;
     const int num_groups = (p.nphase ? p.nphase : 1) * num_tiles;
 
-    if (warp == 0) {
+    if (wg == 2) {
         // ------------------------------------------------------------------ TMA producer
-        {
-            // Executed by the whole warp with warp-uniform control flow; one elected lane issues.  A single thread used to
-            // spend ~1100 cycles per k-block here on index arithmetic (two integer divisions, generic->shared conversions, parameter reloads) -- more than the 128..512 cycles of MMA
-            // work a k-block carries, so EVERY layer ran at the producer's pace (ncu: this warp ~100 % busy, tensor pipe
-            // 11 % / 50 %).  Taps and channel chunks are now nested loops with incremental state; per k-block only the
-            // barrier wait, the expect_tx and the TMA issues remain.
-            const uint32_t smem_base = smem_u32(smem), full0 = smem_u32(full_bar), empty0 = smem_u32(empty_bar);
-            const uint64_t tmB0 = reinterpret_cast<uint64_t>(&p.tmB[0]), tmB1 = reinterpret_cast<uint64_t>(&p.tmB[1]);
-            const int cch = p.cchunks, mode = p.mode, KWv = p.KW, padv = p.pad, stride2 = (p.stride == 2), nph = p.nphase;
-            const int ntap_all = mode == 1 ? p.num_kb / (cch > 0 ? cch : 1) : 0;
-            int stage = 0;
-            uint32_t phase = 0;
-            for (int grp = my_cluster; grp < num_groups; grp += num_clusters) {
-                int rem = grp, tap_base = 0, ntap = ntap_all;
-                if (nph) {
-                    const int ph = grp / num_tiles;
-                    rem = grp - ph * num_tiles;
-                    tap_base = p.ph_tap0[ph];
-                    ntap = p.ph_tap0[ph + 1] - tap_base;
-                }
-                const int n_tile = rem % p.num_n_tiles;
-                const int m_tile = rem / p.num_n_tiles;
-                const int bn0 = n_tile * BLOCK_N;
-                if (mode == 1) {
-                    int n0 = 0, h0 = 0;
-                    if (p.TN == 1) {
-                        n0 = m_tile / p.tiles_per_img;
-                        h0 = (m_tile - n0 * p.tiles_per_img) * p.TH;
-                    } else {
-                        n0 = m_tile * p.TN;
-                    }
-                    int r = 0, s2 = 0;
-                    for (int t = 0; t < ntap; ++t) {
-                        int dh, dw, map = 0, wt = t;
-                        if (nph) {
-                            dh = p.tap_dh[tap_base + t];
-                            dw = p.tap_dw[tap_base + t];
-                            wt = p.tap_w[tap_base + t];
-                        } else {
-                            dh = r - padv;
-                            dw = s2 - padv;
-                            if (stride2) {
-                                map = ((dh & 1) << 1) | (dw & 1);
-                                dh >>= 1;  // arithmetic shift == floor division
-                                dw >>= 1;
-                            }
-                            if (++s2 == KWv) {
-                                s2 = 0;
-                                ++r;
-                            }
-                        }
-                        const uint64_t tmA0 = reinterpret_cast<uint64_t>(&p.tmA[0][map]);
-                        const uint64_t tmA1 = reinterpret_cast<uint64_t>(&p.tmA[1][map]);
-                        const int hh = h0 + dh;
-                        int kw = wt * cch * kBlockK;
-                        for (int cc = 0; cc < cch; ++cc, kw += kBlockK) {
-                            const uint32_t fb = full0 + stage * 8, dst = smem_base + stage * Cfg::STAGE_BYTES;
-                            mbar_wait_u32(empty0 + stage * 8, phase ^ 1);
-                            if (elect_one()) {
-                                mbar_arrive_expect_tx_u32(fb, Cfg::STAGE_BYTES);
-                                tma_load_4d_u32(dst, tmA0, fb, cc * kBlockK, dw, hh, n0);
-                                if (NPL == 2) tma_load_4d_u32(dst + Cfg::A_BYTES, tmA1, fb, cc * kBlockK, dw, hh, n0);
-                                tma_load_2d_u32(dst + NPL * Cfg::A_BYTES, tmB0, fb, kw, bn0);
-                                if (NPL == 2) tma_load_2d_u32(dst + NPL * Cfg::A_BYTES + Cfg::B_BYTES, tmB1, fb, kw, bn0);
-                            }
-                            __syncwarp();
-                            if (++stage == STAGES) {
-                                stage = 0;
-                                phase ^= 1;
-                            }
-                        }
-                    }
+        // Executed by the whole warp with warp-uniform control flow; one elected lane issues.  Taps and channel chunks are
+        // nested loops with incremental state: per k-block only the barrier wait, the expect_tx and the TMA issues remain.
+        const uint32_t smem_base = smem_u32(smem), full0 = smem_u32(full_bar), empty0 = smem_u32(empty_bar);
+        const uint64_t tmB0 = reinterpret_cast<uint64_t>(&p.tmB[0]), tmB1 = reinterpret_cast<uint64_t>(&p.tmB[1]);
+        const int cch = p.cchunks, mode = p.mode, KWv = p.KW, padv = p.pad, stride2 = (p.stride == 2), nph = p.nphase;
+        const int ntap_all = mode == 1 ? p.num_kb / (cch > 0 ? cch : 1) : 0;
+        int stage = 0;
+        uint32_t phase = 0;
+        for (int grp = my_cta; grp < num_groups; grp += num_ctas) {
+            int rem = grp, tap_base = 0, ntap = ntap_all;
+            if (nph) {
+                const int ph = grp / num_tiles;
+                rem = grp - ph * num_tiles;
+                tap_base = p.ph_tap0[ph];
+                ntap = p.ph_tap0[ph + 1] - tap_base;
+            }
+            const int n_tile = rem % p.num_n_tiles;
+            const int m_tile = rem / p.num_n_tiles;
+            const int bn0 = n_tile * BLOCK_N;
+            if (mode == 1) {
+                int n0 = 0, h0 = 0;
+                if (p.TN == 1) {
+                    n0 = m_tile / p.tiles_per_img;
+                    h0 = (m_tile - n0 * p.tiles_per_img) * p.TH;
                 } else {
-                    const uint64_t tmA0 = reinterpret_cast<uint64_t>(&p.tmA[0][0]);
-                    const uint64_t tmA1 = reinterpret_cast<uint64_t>(&p.tmA[1][0]);
-                    const int row0 = m_tile * kBlockM;
-                    for (int kb = 0, kc = 0; kb < p.num_kb; ++kb, kc += kBlockK) {
+                    n0 = m_tile * p.TN;
+                }
+                int r = 0, s2 = 0;
+                for (int t = 0; t < ntap; ++t) {
+                    int dh, dw, map = 0, wt = t;
+                    if (nph) {
+                        dh = p.tap_dh[tap_base + t];
+                        dw = p.tap_dw[tap_base + t];
+                        wt = p.tap_w[tap_base + t];
+                    } else {
+                        dh = r - padv;
+                        dw = s2 - padv;
+                        if (stride2) {
+                            map = ((dh & 1) << 1) | (dw & 1);
+                            dh >>= 1;  // arithmetic shift == floor division
+                            dw >>= 1;
+                        }
+                        if (++s2 == KWv) {
+                            s2 = 0;
+                            ++r;
+                        }
+                    }
+                    const uint64_t tmA0 = reinterpret_cast<uint64_t>(&p.tmA[0][map]);
+                    const uint64_t tmA1 = reinterpret_cast<uint64_t>(&p.tmA[1][map]);
+                    const int hh = h0 + dh;
+                    int kw = wt * cch * kBlockK;
+                    for (int cc = 0; cc < cch; ++cc, kw += kBlockK) {
                         const uint32_t fb = full0 + stage * 8, dst = smem_base + stage * Cfg::STAGE_BYTES;
                         mbar_wait_u32(empty0 + stage * 8, phase ^ 1);
                         if (elect_one()) {
                             mbar_arrive_expect_tx_u32(fb, Cfg::STAGE_BYTES);
-                            tma_load_2d_u32(dst, tmA0, fb, kc, row0);
-                            if (NPL == 2) tma_load_2d_u32(dst + Cfg::A_BYTES, tmA1, fb, kc, row0);
-                            tma_load_2d_u32(dst + NPL * Cfg::A_BYTES, tmB0, fb, kc, bn0);
-                            if (NPL == 2) tma_load_2d_u32(dst + NPL * Cfg::A_BYTES + Cfg::B_BYTES, tmB1, fb, kc, bn0);
+                            tma_load_4d_u32(dst, tmA0, fb, cc * kBlockK, dw, hh, n0);
+                            if (NPL == 2) tma_load_4d_u32(dst + Cfg::A_BYTES, tmA1, fb, cc * kBlockK, dw, hh, n0);
+                            tma_load_2d_u32(dst + NPL * Cfg::A_BYTES, tmB0, fb, kw, bn0);
+                            if (NPL == 2) tma_load_2d_u32(dst + NPL * Cfg::A_BYTES + Cfg::B_BYTES, tmB1, fb, kw, bn0);
                         }
                         __syncwarp();
                         if (++stage == STAGES) {
@@ -227,124 +167,93 @@ __global__ void __launch_bounds__(128 + 32 * kEpiWarps, 1) gemm_fwd_kernel(const
                         }
                     }
                 }
-            }
-        }
-    } else if (warp == 1) {
-        // ------------------------------------------------------------------ MMA issuer
-        {
-            // Executed by the WHOLE warp with warp-uniform control flow; only the tcgen05 instructions are issued by
-            // one elected lane.  (Inside an `if (lane == 0)` region the compiler wraps every UTCHMMA in an ELECT + 5x R2UR
-            // "waterfall" loop, ~20 instructions per MMA.)
-            // The shared-memory descriptors of a stage differ only in their 14-bit address field, so they are
-            // one constant OR-ed with (address >> 4) and advanced by +2 (32 bytes) per 16-wide k-step -- the generic loop
-            // rebuilt eight descriptors per k-block (126 instructions on this single thread).
-            constexpr uint32_t idesc = make_idesc(kBlockM, BLOCK_N, 0, 0);
-            // 3-pass mode: the w_hi and w_lo tiles of a stage are CONTIGUOUS in shared memory (BLOCK_N rows each, same
-            // K-major swizzled layout) and the main / cross accumulators are ADJACENT in TMEM, so a_hi x [w_hi; w_lo] is ONE
-            // MMA of width 2*BLOCK_N writing main | cross.  The kernel is shared-memory-bandwidth bound (TMA writes + MMA
-            // operand reads exceed 128 B/clk): this reads a_hi once instead of twice per k-step (24 -> 20 KB per k-step).
-            constexpr uint32_t idesc_wide = make_idesc(kBlockM, (NSPLIT == 3 ? 2 : 1) * BLOCK_N, 0, 0);
-            static_assert(NSPLIT != 3 || (Cfg::NMAIN == 1 && 2 * BLOCK_N <= 256), "stacked hi|lo MMA needs adjacent accumulators");
-            const uint64_t desc_const = make_smem_desc(0, 16, 1024);
-            const uint32_t smem_base = smem_u32(smem), full0 = smem_u32(full_bar), empty0 = smem_u32(empty_bar);
-            const uint32_t tfull0 = smem_u32(tfull_bar), tempty0 = smem_u32(tempty_bar);
-            const int cch = p.cchunks, nph = p.nphase, nkb_all = p.num_kb;
-            int stage = 0;
-            uint32_t phase = 0;
-            int it = 0;
-            for (int grp = my_cluster; grp < num_groups; grp += num_clusters, ++it) {
-                const int acc = it & 1;
-                mbar_wait_u32(tempty0 + acc * 8, ((it >> 1) & 1) ^ 1);
-                tc_fence_after();
-                const uint32_t d_main = tmem_base + acc * Cfg::NACC * BLOCK_N;
-                const uint32_t d_cross = d_main + Cfg::NMAIN * BLOCK_N;
-                int nkb = nkb_all;
-                if (nph) {
-                    const int ph = grp / num_tiles;
-                    nkb = (p.ph_tap0[ph + 1] - p.ph_tap0[ph]) * cch;
-                }
-                uint32_t accum = 0;
-                for (int kb = 0; kb < nkb; ++kb) {
-                    const uint32_t a_addr = smem_base + stage * Cfg::STAGE_BYTES;
-                    const uint64_t da = desc_const | (uint64_t)(a_addr >> 4);
-                    const uint64_t db = da + ((NPL * Cfg::A_BYTES) >> 4);
-                    mbar_wait_u32(full0 + stage * 8, phase);
-                    tc_fence_after();
+            } else {
+                const uint64_t tmA0 = reinterpret_cast<uint64_t>(&p.tmA[0][0]);
+                const uint64_t tmA1 = reinterpret_cast<uint64_t>(&p.tmA[1][0]);
+                const int row0 = m_tile * kBlockM;
+                for (int kb = 0, kc = 0; kb < p.num_kb; ++kb, kc += kBlockK) {
+                    const uint32_t fb = full0 + stage * 8, dst = smem_base + stage * Cfg::STAGE_BYTES;
+                    mbar_wait_u32(empty0 + stage * 8, phase ^ 1);
                     if (elect_one()) {
-#pragma unroll
-                        for (int k = 0; k < kBlockK / 16; ++k) {
-                            const uint32_t ac = (k == 0) ? accum : 1u;
-                            if (NSPLIT == 3) {
-                                umma_bf16(d_main, da + 2 * k, db + 2 * k, idesc_wide, ac);                    // a_hi x [w_hi; w_lo] -> main | cross
-                                umma_bf16(d_cross, da + (Cfg::A_BYTES >> 4) + 2 * k, db + 2 * k, idesc, 1u);  // a_lo x w_hi -> cross
-                            } else {
-                                umma_bf16(d_main, da + 2 * k, db + 2 * k, idesc, ac);
-                            }
-                        }
-                        umma_commit_u32(empty0 + stage * 8);
+                        mbar_arrive_expect_tx_u32(fb, Cfg::STAGE_BYTES);
+                        tma_load_2d_u32(dst, tmA0, fb, kc, row0);
+                        if (NPL == 2) tma_load_2d_u32(dst + Cfg::A_BYTES, tmA1, fb, kc, row0);
+                        tma_load_2d_u32(dst + NPL * Cfg::A_BYTES, tmB0, fb, kc, bn0);
+                        if (NPL == 2) tma_load_2d_u32(dst + NPL * Cfg::A_BYTES + Cfg::B_BYTES, tmB1, fb, kc, bn0);
                     }
                     __syncwarp();
-                    accum = 1u;
                     if (++stage == STAGES) {
                         stage = 0;
                         phase ^= 1;
                     }
                 }
-                if (elect_one()) umma_commit_u32(tfull0 + acc * 8);
-                __syncwarp();
             }
         }
-    } else if (warp >= 4) {
-        // ------------------------------------------------------------------ epilogue: 2 warpgroups x 128 threads.
-        // Group g drains TMEM accumulator buffer g, i.e. every other tile of this CTA: two tile epilogues are in flight
-        // (needed for small-K layers such as 64->64 3x3, whose 9 k-blocks of MMA are shorter than one epilogue).
-        const int q = warp & 3;  // TMEM lane quadrant this warp may access
-        const int grp = (warp - 4) >> 2;
-        const int row = q * 32 + lane;
-        float* tr = s_tr + (warp - 4) * (32 * 17);
-        // One tile per CTA (small-M layers: 16x16 / 8x8 maps, FC): there is no second tile to overlap with, so both
-        // warpgroups share the single tile's epilogue, each draining half of its column chunks.
-        constexpr int NCH = BLOCK_N / 32;
-        const bool split_epi = num_groups <= num_clusters && !p.no_split_epi;
-        const int c_begin = split_epi ? grp * (NCH / 2) : 0;
-        const int c_end = split_epi ? (grp + 1) * (NCH / 2) : NCH;
-        for (int tg = split_epi ? my_cluster : my_cluster + grp * num_clusters, it = split_epi ? 0 : grp; tg < num_groups;
-             tg += 2 * num_clusters, it += 2) {
-            int rem = tg, ph = 0;
-            if (p.nphase) {
-                ph = tg / num_tiles;
-                rem = tg - ph * num_tiles;
-            }
-            const int n_tile = rem % p.num_n_tiles;
-            const int m_tile = rem / p.num_n_tiles;
-            const int acc = it & 1;
-            const uint32_t acc_phase = (it >> 1) & 1;
-            mbar_wait(&tfull_bar[acc], acc_phase);
-            tc_fence_after();
-            gemm_epilogue_tile<BLOCK_N, NSPLIT, Cfg::NMAIN>(p, tmem_base + ((uint32_t)(q * 32) << 16) + acc * Cfg::NACC * BLOCK_N, lane, row,
-                                                            m_tile, n_tile, ph, c_begin, c_end, tr, s_stats);
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0 && !(split_epi && grp == 1)) mbar_arrive(&tempty_bar[acc]);
-        }
-        if (p.stats != nullptr) {
-            asm volatile("bar.sync 1, 256;" ::: "memory");  // the eight epilogue warps only
-            const int n_tile = my_cluster % p.num_n_tiles;   // fixed per CTA (num_clusters % num_n_tiles == 0)
-            for (int i = threadIdx.x - 128; i < BLOCK_N; i += 256) {
-                const int col = n_tile * BLOCK_N + i;
-                if (col < p.N) {
-                    atomicAdd(p.stats + col, s_stats[i]);
-                    atomicAdd(p.stats + p.N + col, s_stats[BLOCK_N + i]);
-                }
-            }
-        }
+        return;
     }
 
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 2) {
-        tc_fence_after();
-        tmem_dealloc(tmem_base, Cfg::TMEM_COLS);
+    // ---------------------------------------------------------------------- MMA + epilogue warpgroups
+    const int cw = wg;  // rows [64 cw, 64 cw + 64) of every tile
+    const uint64_t desc_const = make_wgmma_desc(0, 16, 1024);
+    const uint32_t smem_base = smem_u32(smem), full0 = smem_u32(full_bar), empty0 = smem_u32(empty_bar);
+    const bool signaller = (threadIdx.x & 127) == 0;
+    const int cch = p.cchunks, nph = p.nphase, nkb_all = p.num_kb;
+    int stage = 0;
+    uint32_t phase = 0;
+    for (int grp = my_cta; grp < num_groups; grp += num_ctas) {
+        int rem = grp, ph = 0, nkb = nkb_all;
+        if (nph) {
+            ph = grp / num_tiles;
+            rem = grp - ph * num_tiles;
+            nkb = (p.ph_tap0[ph + 1] - p.ph_tap0[ph]) * cch;
+        }
+        const int n_tile = rem % p.num_n_tiles;
+        const int m_tile = rem / p.num_n_tiles;
+        float acc[Cfg::ACC_REGS];
+        int prev_stage = -1;
+        for (int kb = 0; kb < nkb; ++kb) {
+            const uint32_t a_addr = smem_base + stage * Cfg::STAGE_BYTES;
+            const uint64_t da = desc_const | (uint64_t)((a_addr + cw * (64 * 128)) >> 4);
+            const uint64_t db = desc_const | (uint64_t)((a_addr + NPL * Cfg::A_BYTES) >> 4);
+            mbar_wait_u32(full0 + stage * 8, phase);
+            wgmma_fence_regs(acc);
+            wgmma_fence();
+#pragma unroll
+            for (int k = 0; k < kBlockK / 16; ++k) {
+                const uint32_t ac = (kb > 0 || k > 0) ? 1u : 0u;
+                if constexpr (NSPLIT == 3) {
+                    Wgmma<BLOCK_N, 0, 0>::mma(acc, da + 2 * k, db + 2 * k, ac);  // a_hi x w_hi -> main
+                    Wgmma<BLOCK_N, 0, 0>::mma(acc + BLOCK_N / 2, da + 2 * k, db + (Cfg::B_BYTES >> 4) + 2 * k, ac);  // a_hi x w_lo -> cross
+                    Wgmma<BLOCK_N, 0, 0>::mma(acc + BLOCK_N / 2, da + (Cfg::A_BYTES >> 4) + 2 * k, db + 2 * k, 1u);  // a_lo x w_hi -> cross
+                } else {
+                    Wgmma<BLOCK_N, 0, 0>::mma(acc, da + 2 * k, db + 2 * k, ac);
+                }
+            }
+            wgmma_commit();
+            wgmma_wait<1>();  // the previous k-block's MMAs are done: its stage may be refilled
+            wgmma_fence_regs(acc);
+            if (prev_stage >= 0 && signaller) mbar_arrive(&empty_bar[prev_stage]);
+            prev_stage = stage;
+            if (++stage == STAGES) {
+                stage = 0;
+                phase ^= 1;
+            }
+        }
+        wgmma_wait<0>();
+        wgmma_fence_regs(acc);
+        if (prev_stage >= 0 && signaller) mbar_arrive(&empty_bar[prev_stage]);
+        gemm_epilogue_tile<BLOCK_N, NSPLIT>(p, acc, lane, cw * 64 + (warp & 3) * 16 + (lane >> 2), m_tile, n_tile, ph, s_stats);
+    }
+    if (p.stats != nullptr) {
+        asm volatile("bar.sync 1, 256;" ::: "memory");  // the two MMA warpgroups only
+        const int n_tile = my_cta % p.num_n_tiles;      // fixed per CTA (num_ctas % num_n_tiles == 0)
+        for (int i = threadIdx.x; i < BLOCK_N; i += 256) {
+            const int col = n_tile * BLOCK_N + i;
+            if (col < p.N) {
+                atomicAdd(p.stats + col, s_stats[i]);
+                atomicAdd(p.stats + p.N + col, s_stats[BLOCK_N + i]);
+            }
+        }
     }
 }
 
@@ -361,21 +270,17 @@ static int launch_gemm(const GemmParams& p, cudaStream_t stream) {
         attr_set = true;
     }
     const int groups = (p.nphase ? p.nphase : 1) * p.num_m_tiles * p.num_n_tiles;
-    int clusters = groups < num_sms() ? groups : num_sms();
-    clusters -= clusters % p.num_n_tiles;  // every CTA keeps one n_tile => per-CTA BatchNorm partial sums
-    if (clusters <= 0) clusters = p.num_n_tiles;
+    int ctas = groups < num_sms() ? groups : num_sms();
+    ctas -= ctas % p.num_n_tiles;  // every CTA keeps one n_tile => per-CTA BatchNorm partial sums
+    if (ctas <= 0) ctas = p.num_n_tiles;
     cudaLaunchConfig_t cfg;
     memset(&cfg, 0, sizeof(cfg));
-    cfg.gridDim = dim3(clusters);
-    cfg.blockDim = dim3(128 + 32 * kEpiWarps);
+    cfg.gridDim = dim3(ctas);
+    cfg.blockDim = dim3(kThreads);
     cfg.dynamicSmemBytes = Cfg::SMEM_BYTES;
     cfg.stream = stream;
-    cudaLaunchAttribute attr[2];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = 1;
-    attr[0].val.clusterDim.y = 1;
-    attr[0].val.clusterDim.z = 1;
-    int na = 1;
+    cudaLaunchAttribute attr[1];
+    int na = 0;
     if (pdl_enabled()) {
         attr[na].id = cudaLaunchAttributeProgrammaticStreamSerialization;
         attr[na].val.programmaticStreamSerializationAllowed = 1;
@@ -390,64 +295,30 @@ static int launch_gemm(const GemmParams& p, cudaStream_t stream) {
 
 static thread_local int g_last_variant = 0;
 
-static int dispatch_gemm(const GemmParams& p_in, int block_n, int nsplit, cudaStream_t stream) {
-    static int no_split = -1;
-    if (no_split < 0) {
-        const char* e = getenv("GDRN_NO_SPLIT_EPI");
-        no_split = e ? atoi(e) : 0;
-    }
-    GemmParams p = p_in;
-    p.no_split_epi = no_split;
+static int dispatch_gemm(const GemmParams& p, int block_n, int nsplit, cudaStream_t stream) {
     g_last_variant = block_n * 10 + nsplit;
     if (nsplit == 1) {
-        if (block_n == 256) return launch_gemm<256, 1>(p, stream);
         if (block_n == 128) return launch_gemm<128, 1>(p, stream);
         if (block_n == 64) return launch_gemm<64, 1>(p, stream);
     } else if (nsplit == 3) {
-        if (block_n == 128) return launch_gemm<128, 3>(p, stream);
         if (block_n == 64) return launch_gemm<64, 3>(p, stream);
     }
     return set_error(GDRN_ERR_ARG, "gemm: unsupported block_n=%d nsplit=%d", block_n, nsplit);
 }
 
 // Tile width: the widest BLOCK_N (fewest A re-reads, best smem-bandwidth ratio) that still yields >= ~0.75 waves of
-// CTAs on the 148 SMs; small-M layers (layer4, FC) fall back to narrower tiles instead of leaving SMs idle.
+// CTAs on the SMs; small-M layers (layer4, FC) fall back to narrower tiles instead of leaving SMs idle.
 static int pick_block_n(int n_pad, int nsplit, int num_m_tiles) {
-    const int want = (num_sms() * 3) / 4;
-    // fp32x3: (main + cross) x 2 buffers x 128 columns = all 512 TMEM columns, so 128 is the widest tile
-    if (nsplit == 1 && n_pad % 256 == 0 && num_m_tiles * (n_pad / 256) >= want) return 256;
-    if (n_pad % 128 == 0 && num_m_tiles * (n_pad / 128) >= want) return 128;
-    if (n_pad % 64 == 0 && num_m_tiles * (n_pad / 128) < num_sms() / 2) return 64;
-    if (n_pad % 128 == 0) return 128;
-    if (n_pad % 64 == 0) return 64;
-    return -1;
-}
-
-// 2-CTA (cta_group::2) pair tiles (gemm_fwd2.cu): 256 x 256 (1 pass) / 256 x 128 (3 pass).  Each CTA stages only half of the
-// weight tile, which takes the kernel off its shared-memory-bandwidth limit (see the header of gemm_fwd2.cu).
-// GDRN_2CTA=0 disables (A/B); layers with an odd tile count or less than half a wave of pair tiles keep the 1-CTA kernel.
-static int g_2cta_mode = -1;
-static std::atomic<long> g_2cta_launches{0};
-static bool want_2cta(int nsplit, int block_n, int num_m_tiles, int num_n_tiles) {
-    if (g_2cta_mode < 0) {
-        const char* e = getenv("GDRN_2CTA");
-        g_2cta_mode = e ? atoi(e) : 1;
-    }
-    if (g_2cta_mode != 1 || (num_m_tiles & 1)) return false;
-    if (!((nsplit == 1 && (block_n == 256 || block_n == 128)) || (nsplit == 3 && block_n == 128))) return false;
-    return (num_m_tiles / 2) * num_n_tiles * 4 >= num_sms();
+    if (n_pad % 64 != 0) return -1;
+    if (nsplit == 3) return 64;  // the widest 3-pass tile that does not spill (see the header comment)
+    if (n_pad % 128 == 0 && num_m_tiles * (n_pad / 128) >= (num_sms() * 3) / 4) return 128;
+    if (num_m_tiles * (n_pad / 128) < num_sms() / 2) return 64;
+    return n_pad % 128 == 0 ? 128 : 64;
 }
 
 }  // namespace gdrn
 
 using namespace gdrn;
-
-// A/B switch: 1 = cta_group::2 pair tiles (gemm_fwd2.cu) for eligible layers (default), 0 = 1-CTA kernel everywhere
-extern "C" int gdrn_set_2cta(int on) {
-    g_2cta_mode = on ? 1 : 0;
-    return 0;
-}
-extern "C" long gdrn_2cta_launch_count() { return gdrn::g_2cta_launches.load(); }
 
 extern "C" int gdrn_conv_fwd(const void* x_hi, const void* x_lo, const void* w_hi, const void* w_lo, void* y_hi,
                              void* y_lo, float* y_f32, const float* bias, const void* res_hi, const void* res_lo, float* stats,
@@ -474,8 +345,6 @@ extern "C" int gdrn_conv_fwd(const void* x_hi, const void* x_lo, const void* w_h
 
     GemmParams p;
     memset(&p, 0, sizeof(p));
-    const bool two_cta = want_2cta(nsplit, block_n, (N * Ho * Wo + 127) / 128, Cout_pad / block_n);
-    const int cluster = two_cta ? 2 : 1;  // 2-CTA pairs: each CTA loads half of the weight tile
     const int npl = nsplit == 1 ? 1 : 2;
     const void* xs[2] = {x_hi, x_lo};
     const void* ws[2] = {w_hi, w_lo};
@@ -492,10 +361,9 @@ extern "C" int gdrn_conv_fwd(const void* x_hi, const void* x_lo, const void* w_h
         }
         uint64_t wdims[2] = {(uint64_t)K, (uint64_t)Cout_pad};
         uint64_t wstr[1] = {(uint64_t)K * 2};
-        uint32_t wbox[2] = {64, (uint32_t)(block_n / cluster)};
+        uint32_t wbox[2] = {64, (uint32_t)block_n};
         if (make_tmap(&p.tmB[pl], ws[pl], 2, wdims, wstr, wbox)) return GDRN_ERR_CUDA;
     }
-    p.cluster = cluster;
     p.mode = 1;
     p.M = N * Ho * Wo;
     p.N = Cout;
@@ -518,11 +386,6 @@ extern "C" int gdrn_conv_fwd(const void* x_hi, const void* x_lo, const void* w_h
     p.res_lo = res_lo;
     p.act = act;
     p.stats = stats;
-    if (two_cta) {
-        g_2cta_launches.fetch_add(1, std::memory_order_relaxed);
-        g_last_variant = 10000 + block_n * 10 + nsplit;  // +10000: the cta_group::2 kernel
-        return launch_gemm_2cta(p, block_n, nsplit, stream);
-    }
     return dispatch_gemm(p, block_n, nsplit, stream);
 }
 
@@ -567,7 +430,6 @@ extern "C" int gdrn_conv_dgrad_s2(const void* du_hi, const void* du_lo, const vo
         uint32_t wbox[2] = {64, (uint32_t)block_n};
         if (make_tmap(&p.tmB[pl], ws[pl], 2, wdims, wstr, wbox)) return GDRN_ERR_CUDA;
     }
-    p.cluster = 1;
     p.mode = 1;
     p.M = N * Ho * Wo;
     p.N = Cx;
@@ -625,7 +487,6 @@ extern "C" int gdrn_gemm_fwd(const void* a_hi, const void* a_lo, const void* w_h
     if (block_n < 0) return set_error(GDRN_ERR_ARG, "gemm_fwd: N_pad=%d must be a multiple of 64", N_pad);
     GemmParams p;
     memset(&p, 0, sizeof(p));
-    const int cluster = 1;
     const int npl = nsplit == 1 ? 1 : 2;
     const void* as[2] = {a_hi, a_lo};
     const void* ws[2] = {w_hi, w_lo};
@@ -635,10 +496,9 @@ extern "C" int gdrn_gemm_fwd(const void* a_hi, const void* a_lo, const void* w_h
         uint32_t abox[2] = {64, 128};
         if (make_tmap(&p.tmA[pl][0], as[pl], 2, adims, astr, abox)) return GDRN_ERR_CUDA;
         uint64_t wdims[2] = {(uint64_t)K, (uint64_t)N_pad};
-        uint32_t wbox[2] = {64, (uint32_t)(block_n / cluster)};
+        uint32_t wbox[2] = {64, (uint32_t)block_n};
         if (make_tmap(&p.tmB[pl], ws[pl], 2, wdims, astr, wbox)) return GDRN_ERR_CUDA;
     }
-    p.cluster = cluster;
     p.mode = 0;
     p.M = M;
     p.N = N;
@@ -655,5 +515,5 @@ extern "C" int gdrn_gemm_fwd(const void* a_hi, const void* a_lo, const void* w_h
     return dispatch_gemm(p, block_n, nsplit, stream);
 }
 
-// BLOCK_N * 10 + NSPLIT (+ 10000 for the cta_group::2 kernel) of the most recent gdrn_conv_fwd / gdrn_gemm_fwd call on this thread
+// BLOCK_N * 10 + NSPLIT of the most recent gdrn_conv_fwd / gdrn_gemm_fwd call on this thread
 extern "C" int gdrn_last_gemm_variant() { return g_last_variant; }

@@ -1,4 +1,4 @@
-// Shared between gemm_fwd.cu (1-CTA tiles) and gemm_fwd2.cu (2-CTA cta_group::2 tiles).
+// Parameters of the implicit-GEMM forward kernel (gemm_fwd.cu) and its epilogue (gemm_epilogue.cuh).
 #pragma once
 #include <cuda.h>
 
@@ -21,7 +21,6 @@ struct GemmParams {
     const void* res_lo;  // the eval-mode folded conv + BN + (identity) + ReLU epilogue of a BasicBlock's second conv
     int act;       // 0 none, 1 LeakyReLU(0.1), 2 ReLU
     float* stats;  // [2][N]: sum, sum of squares (accumulated with atomics) or nullptr
-    int cluster;   // 1, or 2: CTA pairs share one n_tile and each TMA-multicasts half of the weight tile to both
     // Stride-2 dgrad by output-parity phases (mode 1, nphase > 0): rows index the (n, i, j) lattice of dY; phase ph writes
     // output pixel (2i + ph_a, 2j + ph_b) and sums taps [ph_tap0[ph], ph_tap0[ph+1]) of the tables below
     // (dY offset (tap_dh, tap_dw); tap_w = tap slot of the packed weight matrix).  Tiles are enumerated phase-major.
@@ -30,10 +29,6 @@ struct GemmParams {
     int ph_a[4], ph_b[4];
     signed char tap_dh[12], tap_dw[12], tap_w[12];
     int pw_log2, ph_log2;  // log2 of the dY width / height
-    int no_split_epi;      // A/B switch (GDRN_NO_SPLIT_EPI=1): single-tile CTAs keep the whole epilogue on one warpgroup
 };
-
-
-int launch_gemm_2cta(const GemmParams& p, int block_n, int nsplit, cudaStream_t stream);  // gemm_fwd2.cu (block_n = pair tile width)
 
 }  // namespace gdrn

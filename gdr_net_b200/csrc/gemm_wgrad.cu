@@ -1,26 +1,26 @@
-// tcgen05 weight-gradient kernel (sm_100a):  dW[co][tap][ci] = sum_p dY[p][co] * X[p (+) tap][ci]
+// wgmma weight-gradient kernel (sm_90a):  dW[co][tap][ci] = sum_p dY[p][co] * X[p (+) tap][ci]
 //
 // Both operands are "MN-major" for the tensor core: the reduction index is the pixel p, which is the
 // SLOW index of the NHWC tensors, so the 64-pixel x 64-channel TMA boxes land in shared memory as
 // [k = pixel][64 channels = 128 B] rows -- exactly the MN-major 128B-swizzled canonical layout
-// (descriptor a_major = b_major = 1, SBO = 1024 B between 8-pixel groups, LBO = 8192 B between
+// (wgmma transpose flags set, SBO = 1024 B between 8-pixel groups, LBO = 8192 B between
 // 64-channel chunks).  No transposes are ever materialised.
 //
 //   * A tile = dY  [64 pixels][128 co]      (2 boxes of 64 channels, plain 2-D view [P][Cout])
 //   * B tile = X   [64 pixels][<=256 ci]    (<=4 boxes; for a conv the box is the tap-shifted 4-D
 //                  window of the NHWC input, zero-filled outside the image; stride-2 convs read the
 //                  four parity sub-lattices, like the forward kernel)
-//   * one CTA = (co tile, ci tile, tap, K-split); fp32 accumulator in TMEM (<=256 columns);
-//     partial results go to a [ksplit][Cout][taps*Cin] fp32 workspace that the unpack kernel
-//     (pack.cu) reduces and transposes into the reference's OIHW gradient layout.
+//   * one CTA = (co tile, ci tile, tap, K-split); warpgroups 0 and 1 each own 64 output channels (one dY
+//     box) with fp32 accumulators in registers, warp 8 is the TMA producer; partial results go to a
+//     [ksplit][Cout][taps*Cin] fp32 workspace that the unpack kernel (pack.cu) reduces and transposes
+//     into the reference's OIHW gradient layout.
 // Backward call sites replaced: autograd wgrad of every nn.Conv2d / ConvTranspose2d / nn.Linear in
 // reference resnet_backbone.py, cdpn_rot_head_region.py, conv_pnp_net.py (cuDNN/cuBLAS today).
 #include <stdlib.h>
 
-#include <atomic>
-
 #include "gdrn_internal.h"
 #include "ptx.cuh"
+#include "wgmma.cuh"
 
 namespace gdrn {
 
@@ -41,7 +41,7 @@ struct WgradParams {
 };
 
 constexpr int kWgStageA = 2 * 8192;
-constexpr int kWgThreads = 64 + 256;  // warp 0 TMA, warp 1 MMA + TMEM alloc, warps 2-9: two epilogue warpgroups (column halves)
+constexpr int kWgThreads = 288;  // warps 0-7: two MMA warpgroups (64 output channels each), warp 8: TMA producer
 
 template <int N_TILE, int NSPLIT>
 struct WgradCfg {
@@ -53,12 +53,9 @@ struct WgradCfg {
     static constexpr int STAGES_RAW = (227 * 1024 - 2048) / STAGE_BYTES;
     static constexpr int STAGES = STAGES_RAW > 6 ? 6 : STAGES_RAW;
     static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 2048;
-    // round-toward-zero accumulation (see gemm_fwd.cu): cross terms and three round-robin hi*hi partials
-    static constexpr int NMAIN = (NSPLIT == 3) ? 3 : 1;
-    static constexpr int NACC = (NSPLIT == 3) ? 4 : 1;
-    static constexpr int TMEM_RAW = NACC * N_TILE;
-    static constexpr int TMEM_COLS = TMEM_RAW <= 32 ? 32 : TMEM_RAW <= 64 ? 64 : TMEM_RAW <= 128 ? 128 : TMEM_RAW <= 256 ? 256 : 512;
-    static_assert(NACC * N_TILE <= 512, "TMEM overflow");
+    // 3-pass mode: the cross terms get their own accumulator, added with a round-to-nearest fp32 fma in the epilogue
+    static constexpr int NACC = (NSPLIT == 3) ? 2 : 1;
+    static constexpr int ACC = N_TILE / 2;  // registers per accumulator set: 64 rows x N_TILE columns over 128 threads
     static_assert(STAGES >= 2, "pipeline too shallow");
 };
 
@@ -70,12 +67,10 @@ __global__ void __launch_bounds__(kWgThreads, 1) gemm_wgrad_kernel(const __grid_
     constexpr int NCH = Cfg::NCH;
 
     extern __shared__ uint8_t smem_raw[];
-    uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+    uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
     uint8_t* aux = smem + STAGES * Cfg::STAGE_BYTES;
     uint64_t* full_bar = reinterpret_cast<uint64_t*>(aux);
     uint64_t* empty_bar = full_bar + STAGES;
-    uint64_t* done_bar = empty_bar + STAGES;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(done_bar + 1);
 
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
@@ -93,30 +88,20 @@ __global__ void __launch_bounds__(kWgThreads, 1) gemm_wgrad_kernel(const __grid_
     const int kb_end = min(p.kb_total, kb_begin + kb_per);
     const int nkb = kb_end - kb_begin;  // may be <= 0 for a ragged last split: then we store zeros
 
-    if (warp == 0 && lane == 0) {
+    if (threadIdx.x == 0) {
         for (int s = 0; s < STAGES; ++s) {
             mbar_init(&full_bar[s], 1);
-            mbar_init(&empty_bar[s], 1);
+            mbar_init(&empty_bar[s], 2);  // one arrival per MMA warpgroup
         }
-        mbar_init(done_bar, 1);
         fence_barrier_init();
     }
-    if (warp == 1) {
-        tmem_alloc(tmem_slot, Cfg::TMEM_COLS);
-        tmem_relinquish();
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
     pdl_launch_dependents();  // the next kernel of the stream may start its prologue under our tail
     pdl_wait();               // nothing above touched global memory; from here on we read what the predecessor wrote
 
-    // Producer and MMA issuer run their loops with the WHOLE warp (warp-uniform control flow, operands in uniform registers);
-    // one elected lane issues the TMA / tcgen05 instructions.  Per k-block nothing but the barrier wait, the expect_tx and the
-    // issues remains (the first version rebuilt coordinates with divisions and eight descriptors per k-block on one thread,
-    // which -- not the tensor pipe -- set the pace; see gemm_fwd.cu).
-    if (warp == 0) {
+    if (warp == 8) {
+        // TMA producer: the whole warp runs the loop (warp-uniform control flow, operands in uniform registers), one elected
+        // lane issues; per k-block nothing but the barrier wait, the expect_tx and the issues remains.
         if (nkb > 0) {
             int dh = 0, dw = 0, map = 0;
             if (p.mode == 1 && p.tap_pack) {
@@ -195,347 +180,71 @@ __global__ void __launch_bounds__(kWgThreads, 1) gemm_wgrad_kernel(const __grid_
                 }
             }
         }
-    } else if (warp == 1) {
-        if (nkb > 0) {
-            constexpr uint32_t idesc = make_idesc(128, N_TILE, 1, 1);
-            const uint64_t desc_const = make_smem_desc(0, 8192, 1024);  // only the 14-bit address field varies
-            const uint32_t smem_base = smem_u32(smem), full0 = smem_u32(full_bar), empty0 = smem_u32(empty_bar);
-            int stage = 0, main_idx = 0;
-            uint32_t phase = 0;
-            for (int kb = 0; kb < nkb; ++kb) {
-                const uint32_t a_addr = smem_base + stage * Cfg::STAGE_BYTES;
-                const uint64_t da = desc_const | (uint64_t)(a_addr >> 4);
-                const uint64_t db = da + ((NPL * Cfg::A_BYTES) >> 4);
-                mbar_wait_u32(full0 + stage * 8, phase);
-                tc_fence_after();
-                if (elect_one()) {
+        return;
+    }
+
+    // ---------------------------------------------------------------------- MMA + epilogue warpgroups
+    const int cw = threadIdx.x >> 7;  // output channels [64 cw, 64 cw + 64) of the tile = dY box cw
+    float acc[Cfg::NACC * Cfg::ACC];
+    if (nkb > 0) {
+        const uint64_t desc_const = make_wgmma_desc(0, 8192, 1024);  // only the 14-bit address field varies
+        const uint32_t smem_base = smem_u32(smem), full0 = smem_u32(full_bar);
+        const bool signaller = (threadIdx.x & 127) == 0;
+        int stage = 0, prev_stage = -1;
+        uint32_t phase = 0;
+        for (int kb = 0; kb < nkb; ++kb) {
+            const uint32_t a_addr = smem_base + stage * Cfg::STAGE_BYTES;
+            const uint64_t da = desc_const | (uint64_t)((a_addr + cw * 8192) >> 4);
+            const uint64_t db = desc_const | (uint64_t)((a_addr + NPL * Cfg::A_BYTES) >> 4);
+            mbar_wait_u32(full0 + stage * 8, phase);
+            wgmma_fence_regs(acc);
+            wgmma_fence();
 #pragma unroll
-                    for (int k = 0; k < 4; ++k) {  // 16 pixels (= 16 rows of 128 B = 2048 B) per MMA
-                        if (NSPLIT == 3) {
-                            umma_bf16(tmem_base + main_idx * N_TILE, da + 128 * k, db + 128 * k, idesc,
-                                      (kb >= Cfg::NMAIN || k != 0) ? 1u : 0u);
-                            umma_bf16(tmem_base + Cfg::NMAIN * N_TILE, da + 128 * k, db + (Cfg::B_BYTES >> 4) + 128 * k, idesc,
-                                      (kb | k) != 0 ? 1u : 0u);
-                            umma_bf16(tmem_base + Cfg::NMAIN * N_TILE, da + (Cfg::A_BYTES >> 4) + 128 * k, db + 128 * k, idesc, 1u);
-                        } else {
-                            umma_bf16(tmem_base, da + 128 * k, db + 128 * k, idesc, (kb | k) != 0 ? 1u : 0u);
-                        }
-                    }
-                    umma_commit_u32(empty0 + stage * 8);
-                }
-                __syncwarp();
-                if (++main_idx == Cfg::NMAIN) main_idx = 0;
-                if (++stage == STAGES) {
-                    stage = 0;
-                    phase ^= 1;
+            for (int k = 0; k < 4; ++k) {  // 16 pixels (= 16 rows of 128 B = 2048 B) per MMA
+                const uint32_t ac = (kb | k) != 0 ? 1u : 0u;
+                Wgmma<N_TILE, 1, 1>::mma(acc, da + 128 * k, db + 128 * k, ac);
+                if constexpr (NSPLIT == 3) {
+                    Wgmma<N_TILE, 1, 1>::mma(acc + Cfg::ACC, da + 128 * k, db + (Cfg::B_BYTES >> 4) + 128 * k, ac);  // hi x lo
+                    Wgmma<N_TILE, 1, 1>::mma(acc + Cfg::ACC, da + (Cfg::A_BYTES >> 4) + 128 * k, db + 128 * k, 1u);  // lo x hi
                 }
             }
-            if (elect_one()) umma_commit(done_bar);
-            __syncwarp();
+            wgmma_commit();
+            wgmma_wait<1>();  // the previous k-block's MMAs are done: its stage may be refilled
+            wgmma_fence_regs(acc);
+            if (prev_stage >= 0 && signaller) mbar_arrive(&empty_bar[prev_stage]);
+            prev_stage = stage;
+            if (++stage == STAGES) {
+                stage = 0;
+                phase ^= 1;
+            }
         }
+        wgmma_wait<0>();
+        wgmma_fence_regs(acc);
     } else {
-        // epilogue warps 2..9: TMEM lane quadrant = warp % 4; the CTA's single tile is drained by two warpgroups, each
-        // taking half of the 32-column chunks (one work item per CTA: the epilogue is fully exposed)
-        const int q = warp & 3;
-        const int half = (warp - 2) >> 2;
-        const int row = q * 32 + lane;
-        const int co = m_tile * 128 + row;
-        if (nkb > 0) {
-            mbar_wait(done_bar, 0);
-            tc_fence_after();
-        }
-        const size_t ld = (size_t)p.ws_ld;
-        // tap_pack: columns (filter column, ci) of filter row `tap` are contiguous in the [co][tap][ci] workspace row
-        const size_t col0 = p.tap_pack ? (size_t)tap * N_TILE : (size_t)tap * p.Ntot + (size_t)n_tile * N_TILE;
+#pragma unroll
+        for (int i = 0; i < Cfg::NACC * Cfg::ACC; ++i) acc[i] = 0.f;
+    }
+    // fragment layout (wgmma.cuh): acc[4j + 2h + e] = channel row (warp % 4) * 16 + lane / 4 + 8h, column 8j + 2 (lane % 4) + e
+    const size_t ld = (size_t)p.ws_ld;
+    // tap_pack: columns (filter column, ci) of filter row `tap` are contiguous in the [co][tap][ci] workspace row
+    const size_t col0 = p.tap_pack ? (size_t)tap * N_TILE : (size_t)tap * p.Ntot + (size_t)n_tile * N_TILE;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+        const int co = m_tile * 128 + cw * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * h;
         float* dst_row = p.ws + ((size_t)ks * p.num_m_tiles * 128 + co) * ld + col0;
-#pragma unroll 1
-        for (int c = half * (N_TILE / 64); c < (half + 1) * (N_TILE / 64); ++c) {
-            uint32_t raw[32];
-            if (nkb > 0) {
-                const uint32_t t0 = tmem_base + ((uint32_t)(q * 32) << 16) + c * 32;
-                tmem_ld_32x32(t0, raw);
-                tmem_ld_wait();
-                if (NSPLIT == 3) {
-                    const int nmain = nkb < Cfg::NMAIN ? nkb : Cfg::NMAIN;
-                    for (int a2 = 1; a2 <= Cfg::NMAIN; ++a2) {
-                        if (a2 < Cfg::NMAIN && a2 >= nmain) continue;
-                        uint32_t r2[32];
-                        tmem_ld_32x32(t0 + a2 * N_TILE, r2);
-                        tmem_ld_wait();
 #pragma unroll
-                        for (int j = 0; j < 32; ++j)
-                            raw[j] = __float_as_uint(fmaf(__uint_as_float(r2[j]), a2 == Cfg::NMAIN ? kLoInvScale : 1.f, __uint_as_float(raw[j])));
-                    }
-                }
-            } else {
+        for (int j = 0; j < N_TILE / 8; ++j) {
+            const int cl = 8 * j + 2 * (lane & 3);
+            if (!p.tap_pack && n_tile * N_TILE + cl >= p.Ntot) continue;
+            float v[2];
 #pragma unroll
-                for (int j = 0; j < 32; ++j) raw[j] = 0u;
+            for (int e = 0; e < 2; ++e) {
+                v[e] = acc[4 * j + 2 * h + e];
+                if (NSPLIT == 3) v[e] = fmaf(acc[Cfg::ACC + 4 * j + 2 * h + e], kLoInvScale, v[e]);
             }
-            if (p.tap_pack || n_tile * N_TILE + c * 32 < p.Ntot) {
-#pragma unroll
-                for (int j = 0; j < 32; j += 4)
-                    *reinterpret_cast<uint4*>(dst_row + c * 32 + j) = make_uint4(raw[j], raw[j + 1], raw[j + 2], raw[j + 3]);
-            }
+            *reinterpret_cast<float2*>(dst_row + cl) = make_float2(v[0], v[1]);
         }
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) {
-        tc_fence_after();
-        tmem_dealloc(tmem_base, Cfg::TMEM_COLS);
-    }
-}
-
-// ------------------------------------------------------------------------------------------------
-// cta_group::2 variant (single-plane operands): a CTA PAIR owns one 256 (co) x N_TILE (ci) tile of a (tap, K-split) work item.
-// Same reasoning as gemm_fwd2.cu: per 64-pixel k-block the 1-CTA kernel's shared memory serves 48 KB of TMA writes + 4 x 12 KB
-// of MMA operand reads = 96 KB for 512 MMA cycles (187 B/clk against 128 B/clk); in a pair each CTA stages its own 128 output
-// channels of dY but only HALF of the X columns: 32 KB + 4 x 8 KB = 64 KB (125 B/clk).  Eligible: Cout a multiple of 256 (head,
-// layer3, layer4, deconv), no tap packing.  Identical arithmetic / accumulation order to the 1-CTA kernel (bit-equal, tested).
-// MEASURED (profiles/r2_wgrad_2cta_ab.txt): alone under ncu the two long-K head layers go from 76 % to 84 % tensor pipe (210 ->
-// 197 us), every short-K layer (layer3 / layer4, 32 k-blocks per CTA) stays at 33 % -- those are bound by the fixed cost per
-// work item (prologue + 128 KB fp32 partial per CTA + its unpack), not by shared memory.  In the real step the pair kernel runs
-// on the weight-gradient side stream next to main-stream kernels, where a cluster needs BOTH SMs of a TPC free at once: A/B
-// 10.99 / 10.93 ms (off) vs 11.05 / 11.00 ms (on).  Hence default OFF; GDRN_WGRAD_2CTA=1 / gdrn_set_wgrad_2cta(1) enables it.
-template <int N_TILE>
-struct Wgrad2Cfg {
-    static constexpr int NCH = N_TILE / 64;      // 64-column chunks of the pair tile
-    static constexpr int NCH_H = NCH / 2;        // chunks staged by one CTA
-    static constexpr int A_BYTES = kWgStageA;    // dY [64 px][128 co]
-    static constexpr int B_BYTES = NCH_H * 8192;  // X  [64 px][N_TILE / 2 ci]
-    static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-    static constexpr int STAGES_RAW = (227 * 1024 - 2048) / STAGE_BYTES;
-    static constexpr int STAGES = STAGES_RAW > 8 ? 8 : STAGES_RAW;
-    static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 2048;
-    static_assert(NCH % 2 == 0 && N_TILE <= 256, "pair tile: 128 or 256 input channels");
-};
-
-template <int N_TILE>
-__global__ void __launch_bounds__(kWgThreads, 1) gemm_wgrad2_kernel(const __grid_constant__ WgradParams p) {
-    using Cfg = Wgrad2Cfg<N_TILE>;
-    constexpr int STAGES = Cfg::STAGES;
-    constexpr int NCH_H = Cfg::NCH_H;
-
-    extern __shared__ uint8_t smem_raw[];
-    uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-    uint8_t* aux = smem + STAGES * Cfg::STAGE_BYTES;
-    uint64_t* full_bar = reinterpret_cast<uint64_t*>(aux);  // leader only
-    uint64_t* empty_bar = full_bar + STAGES;                // per CTA
-    uint64_t* done_bar = empty_bar + STAGES;                // per CTA (multicast commit)
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(done_bar + 1);
-
-    const int warp = threadIdx.x >> 5;
-    const int lane = threadIdx.x & 31;
-    const uint32_t crank = cluster_ctarank();
-    const bool leader = crank == 0;
-
-    // work item decode (per PAIR): m pair fastest, then n, tap, ksplit
-    int item = blockIdx.x >> 1;
-    const int m_pairs = p.num_m_tiles / 2;
-    const int m_tile = (item % m_pairs) * 2 + (int)crank;
-    item /= m_pairs;
-    const int n_tile = item % p.num_n_tiles;
-    item /= p.num_n_tiles;
-    const int tap = item % p.items;
-    const int ks = item / p.items;
-    const int kb_per = (p.kb_total + p.ksplit - 1) / p.ksplit;
-    const int kb_begin = ks * kb_per;
-    const int kb_end = min(p.kb_total, kb_begin + kb_per);
-    const int nkb = kb_end - kb_begin;
-
-    if (warp == 0 && lane == 0) {
-        for (int s = 0; s < STAGES; ++s) {
-            mbar_init(&full_bar[s], 1);
-            mbar_init(&empty_bar[s], 1);
-        }
-        mbar_init(done_bar, 1);
-        fence_barrier_init();
-    }
-    if (warp == 1) {
-        asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(N_TILE <= 128 ? 128 : 256)
-                     : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-    }
-    tc_fence_before();
-    __syncthreads();
-    cluster_sync_all();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
-    pdl_launch_dependents();  // the next kernel of the stream may start its prologue under our tail
-    pdl_wait();               // nothing above touched global memory; from here on we read what the predecessor wrote
-
-    if (warp == 0) {
-        if (nkb > 0) {
-            int dh = 0, dw = 0, map = 0;
-            if (p.mode == 1) {
-                const int r = tap / p.KW;
-                const int s2 = tap - r * p.KW;
-                dh = r - p.pad;
-                dw = s2 - p.pad;
-                if (p.stride == 2) {
-                    map = ((dh & 1) << 1) | (dw & 1);
-                    dh >>= 1;
-                    dw >>= 1;
-                }
-            }
-            const uint32_t smem_base = smem_u32(smem), empty0 = smem_u32(empty_bar);
-            const uint32_t full0_local = smem_u32(full_bar), full0 = mapa_cta0(full0_local);
-            const uint64_t tmA0 = reinterpret_cast<uint64_t>(&p.tmA[0]);
-            const uint64_t tmB0 = reinterpret_cast<uint64_t>(&p.tmB[0][map]);
-            const int mode = p.mode, bpi = p.blocks_per_img, THk = p.THk, TNk = p.TNk;
-            const int m0 = m_tile * 128, nb0 = n_tile * N_TILE + (int)crank * (N_TILE / 2);
-            int n0 = 0, hb = 0;
-            if (mode == 1) {
-                if (TNk == 1) {
-                    n0 = kb_begin / bpi;
-                    hb = kb_begin - n0 * bpi;
-                } else {
-                    n0 = kb_begin * TNk;
-                }
-            }
-            int stage = 0;
-            uint32_t phase = 0;
-            for (int kb = kb_begin; kb < kb_end; ++kb) {
-                const uint32_t fb = full0 + stage * 8, dst = smem_base + stage * Cfg::STAGE_BYTES;
-                const int hh = hb * THk + dh, prow = kb * 64;
-                mbar_wait_u32(empty0 + stage * 8, phase ^ 1);
-                if (elect_one()) {
-                    if (leader) mbar_arrive_expect_tx_u32(full0_local + stage * 8, 2 * Cfg::STAGE_BYTES);  // both CTAs' bytes
-                    tma2_load_2d_u32(dst, tmA0, fb, m0, prow);
-                    tma2_load_2d_u32(dst + 8192, tmA0, fb, m0 + 64, prow);
-                    const uint32_t b_dst = dst + Cfg::A_BYTES;
-                    if (mode == 1) {
-#pragma unroll
-                        for (int c = 0; c < NCH_H; ++c) tma2_load_4d_u32(b_dst + c * 8192, tmB0, fb, nb0 + c * 64, dw, hh, n0);
-                    } else {
-#pragma unroll
-                        for (int c = 0; c < NCH_H; ++c) tma2_load_2d_u32(b_dst + c * 8192, tmB0, fb, nb0 + c * 64, prow);
-                    }
-                }
-                __syncwarp();
-                if (mode == 1) {
-                    if (TNk == 1) {
-                        if (++hb == bpi) {
-                            hb = 0;
-                            ++n0;
-                        }
-                    } else {
-                        n0 += TNk;
-                    }
-                }
-                if (++stage == STAGES) {
-                    stage = 0;
-                    phase ^= 1;
-                }
-            }
-        }
-    } else if (warp == 1) {
-        if (leader && nkb > 0) {
-            constexpr uint32_t idesc = make_idesc(256, N_TILE, 1, 1);
-            const uint64_t desc_const = make_smem_desc(0, 8192, 1024);
-            const uint32_t smem_base = smem_u32(smem), full0 = smem_u32(full_bar), empty0 = smem_u32(empty_bar);
-            int stage = 0;
-            uint32_t phase = 0;
-            for (int kb = 0; kb < nkb; ++kb) {
-                const uint32_t a_addr = smem_base + stage * Cfg::STAGE_BYTES;
-                const uint64_t da = desc_const | (uint64_t)(a_addr >> 4);
-                const uint64_t db = da + (Cfg::A_BYTES >> 4);
-                mbar_wait_u32(full0 + stage * 8, phase);
-                tc_fence_after();
-                if (elect_one()) {
-#pragma unroll
-                    for (int k = 0; k < 4; ++k) umma2(tmem_base, da + 128 * k, db + 128 * k, idesc, (kb | k) != 0 ? 1u : 0u);
-                    umma2_commit_u32(empty0 + stage * 8);
-                }
-                __syncwarp();
-                if (++stage == STAGES) {
-                    stage = 0;
-                    phase ^= 1;
-                }
-            }
-            if (elect_one()) umma2_commit_u32(smem_u32(done_bar));
-            __syncwarp();
-        }
-    } else {
-        const int q = warp & 3;
-        const int half = (warp - 2) >> 2;
-        const int row = q * 32 + lane;
-        const int co = m_tile * 128 + row;
-        if (nkb > 0) {
-            mbar_wait(done_bar, 0);
-            tc_fence_after();
-        }
-        const size_t ld = (size_t)p.ws_ld;
-        const size_t col0 = (size_t)tap * p.Ntot + (size_t)n_tile * N_TILE;
-        float* dst_row = p.ws + ((size_t)ks * p.num_m_tiles * 128 + co) * ld + col0;
-#pragma unroll 1
-        for (int c = half * (N_TILE / 64); c < (half + 1) * (N_TILE / 64); ++c) {
-            uint32_t raw[32];
-            if (nkb > 0) {
-                tmem_ld_32x32(tmem_base + ((uint32_t)(q * 32) << 16) + c * 32, raw);
-                tmem_ld_wait();
-            } else {
-#pragma unroll
-                for (int j = 0; j < 32; ++j) raw[j] = 0u;
-            }
-            if (n_tile * N_TILE + c * 32 < p.Ntot) {
-#pragma unroll
-                for (int j = 0; j < 32; j += 4)
-                    *reinterpret_cast<uint4*>(dst_row + c * 32 + j) = make_uint4(raw[j], raw[j + 1], raw[j + 2], raw[j + 3]);
-            }
-        }
-    }
-    tc_fence_before();
-    __syncthreads();
-    cluster_sync_all();  // the peer may not exit (or free TMEM) while the leader's MMAs still read its smem / write its TMEM
-    if (warp == 1) {
-        tc_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(N_TILE <= 128 ? 128 : 256) : "memory");
-    }
-}
-
-template <int N_TILE>
-static int launch_wgrad2(const WgradParams& p, cudaStream_t stream) {
-    using Cfg = Wgrad2Cfg<N_TILE>;
-    auto kern = gemm_wgrad2_kernel<N_TILE>;
-    static bool attr_set = false;
-    if (!attr_set) {
-        GDRN_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
-        attr_set = true;
-    }
-    cudaLaunchConfig_t cfg;
-    memset(&cfg, 0, sizeof(cfg));
-    cfg.gridDim = dim3(p.num_m_tiles * p.num_n_tiles * p.items * p.ksplit);  // (m_tiles / 2) pairs x 2 CTAs
-    cfg.blockDim = dim3(kWgThreads);
-    cfg.dynamicSmemBytes = Cfg::SMEM_BYTES;
-    cfg.stream = stream;
-    cudaLaunchAttribute attr[2];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = 2;
-    attr[0].val.clusterDim.y = 1;
-    attr[0].val.clusterDim.z = 1;
-    int na = 1;
-    if (pdl_enabled()) {
-        attr[na].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-        attr[na].val.programmaticStreamSerializationAllowed = 1;
-        ++na;
-    }
-    cfg.attrs = attr;
-    cfg.numAttrs = na;
-    GDRN_CUDA_OK(cudaLaunchKernelEx(&cfg, kern, p));
-    count_launch();
-    return 0;
-}
-
-static int g_wgrad_2cta = -1;  // GDRN_WGRAD_2CTA=1 enables the pair kernel (default off: neutral-to-slower in situ, see header comment)
-static std::atomic<long> g_wgrad_2cta_launches{0};
-static bool want_wgrad_2cta(const WgradParams& p, int n_tile, int nsplit) {
-    if (g_wgrad_2cta < 0) {
-        const char* e = getenv("GDRN_WGRAD_2CTA");
-        g_wgrad_2cta = e ? atoi(e) : 0;
-    }
-    return g_wgrad_2cta == 1 && nsplit == 1 && !p.tap_pack && (p.num_m_tiles % 2) == 0 && (n_tile == 256 || n_tile == 128) &&
-           (p.Mvalid % 256) == 0;
 }
 
 template <int N_TILE, int NSPLIT>
@@ -568,10 +277,6 @@ static int launch_wgrad(const WgradParams& p, cudaStream_t stream) {
 }
 
 static int dispatch_wgrad(const WgradParams& p, int n_tile, int nsplit, cudaStream_t stream) {
-    if (want_wgrad_2cta(p, n_tile, nsplit)) {
-        g_wgrad_2cta_launches.fetch_add(1, std::memory_order_relaxed);
-        return n_tile == 256 ? launch_wgrad2<256>(p, stream) : launch_wgrad2<128>(p, stream);
-    }
     if (nsplit == 1) {
         if (n_tile == 256) return launch_wgrad<256, 1>(p, stream);
         if (n_tile == 192) return launch_wgrad<192, 1>(p, stream);
@@ -599,7 +304,7 @@ using namespace gdrn;
 static int choose_ksplit(int base_items, int kb_total, int requested) {
     if (requested > 0) return requested < kb_total ? requested : kb_total;
     // one full wave of CTAs (each CTA is one (tile, tap, K-split) work item and owns an SM: 1 CTA/SM by smem), with at
-    // least 8 k-blocks per split so the pipeline fill / TMEM drain is amortised
+    // least 8 k-blocks per split so the pipeline fill / epilogue is amortised
     int ks = num_sms() / base_items;
     int max_ks = kb_total / 8;
     if (max_ks < 1) max_ks = 1;
@@ -607,12 +312,6 @@ static int choose_ksplit(int base_items, int kb_total, int requested) {
     if (ks < 1) ks = 1;
     return ks;
 }
-
-extern "C" int gdrn_set_wgrad_2cta(int on) {
-    gdrn::g_wgrad_2cta = on ? 1 : 0;
-    return 0;
-}
-extern "C" long gdrn_wgrad_2cta_launch_count() { return gdrn::g_wgrad_2cta_launches.load(); }
 
 extern "C" int gdrn_conv_wgrad(const void* dy_hi, const void* dy_lo, const void* x_hi, const void* x_lo, float* ws,
                                long ws_floats, long* ws_need_out, int* ksplit_out, int N, int H, int W, int Cin, int Cout, int KH, int KW,

@@ -3,8 +3,8 @@
 // kernels x 148 tensors per step), and the multi-tensor torch._foreach restatement of round 1.
 //
 // HBM-bound: per step the kernel reads g, p, m, v and writes p, m, v once (28 B / parameter; +8 B on the every-k-th
-// lookahead step); the centralisation's second read of a gradient row hits L1/L2.  35.05 M parameters -> 0.98 GB -> ~0.15 ms
-// at the measured 6.57 TB/s.
+// lookahead step); the centralisation's second read of a gradient row hits L1/L2.  35.05 M parameters -> 0.98 GB -> ~0.3 ms
+// at H100 HBM3 bandwidth.
 //
 // Work decomposition: a device-resident table of per-tensor jobs and a flat list of block descriptors built once by the
 // host (gdr_net_b200/solver.py).  Tensors with dim > 1 are centralised per output row (mean over dims 1..): rows of up to

@@ -200,7 +200,7 @@ __global__ void __launch_bounds__(256) unpack_wgrad_kernel(const float* __restri
         }
     } else {
         // 16-byte loads (IC, ipad, krow and the split stride are multiples of 4 floats -- checked by the host): with one
-        // request per thread in flight, 4-byte loads cap an SM at ~8 KB outstanding (~1.7 TB/s of L2 reads over 148 SMs).
+        // request per thread in flight, 4-byte loads cap an SM at ~8 KB outstanding (~1.5 TB/s of L2 reads over 132 SMs).
         const int ic4 = IC >> 2;
         const int nvec = taps * ic4;
         const float inv_nvec = 1.f / (float)nvec, inv_ic4 = 1.f / (float)ic4;

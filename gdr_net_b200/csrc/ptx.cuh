@@ -1,6 +1,6 @@
-// sm_100a PTX wrappers used by the tcgen05 kernels: mbarrier, TMA (cp.async.bulk.tensor),
-// tcgen05 alloc / mma / commit / ld, descriptors.  Hand-written inline PTX; bit layouts follow
-// the PTX ISA "tcgen05 matrix/instruction descriptor" tables.
+// sm_90a PTX wrappers used by the GEMM kernels: mbarrier, TMA (cp.async.bulk.tensor), wgmma fences and
+// shared-memory matrix descriptors (the MMA itself is in wgmma.cuh).  Hand-written inline PTX; the descriptor
+// layout follows the PTX ISA "matrix descriptor format" table of the wgmma section.
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -99,33 +99,17 @@ __device__ __forceinline__ void tma_load_4d_u32(uint32_t dst, uint64_t tmap, uin
         ::"r"(dst), "l"(tmap), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
         : "memory");
 }
-__device__ __forceinline__ void umma_commit_u32(uint32_t bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
 
-// multicast variant: the box lands at the same smem offset in every CTA of `cta_mask` and completes tx bytes on the
-// mbarrier at the same offset in each of them
-__device__ __forceinline__ void tma_load_2d_mcast(void* smem_dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1,
-                                                  uint16_t cta_mask) {
-    asm volatile(
-        "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, {%3, %4}], "
-        "[%2], %5;"
-        ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "h"(cta_mask)
-        : "memory");
-}
 __device__ __forceinline__ uint32_t cluster_ctarank() {
     uint32_t r;
     asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
     return r;
 }
-__device__ __forceinline__ void cluster_sync_all() {
-    asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
 
 // ---------------------------------------------------------------- programmatic dependent launch
 // A kernel launched with cudaLaunchAttributeProgrammaticStreamSerialization may start while its predecessor in the stream is
 // still running; `pdl_wait` blocks until that predecessor has COMPLETED and its memory is visible.  Everything before it
-// (barrier init, TMEM allocation, descriptor prefetch) overlaps the predecessor's tail.  `pdl_launch_dependents` lets the NEXT
+// (barrier init, descriptor prefetch) overlaps the predecessor's tail.  `pdl_launch_dependents` lets the NEXT
 // kernel of the stream begin that early start; it is always safe because the next kernel protects itself with its own wait.
 // Both are no-ops when the launch carries no programmatic dependency.
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
@@ -138,120 +122,38 @@ __device__ __forceinline__ void pdl_ew_entry() {
     pdl_wait();
 }
 
-// ---------------------------------------------------------------- cta_group::2 (CTA pairs)
-// cp.async.bulk.tensor issued by EITHER CTA of the pair; the transaction bytes are counted on the LEADER's barrier
-// (`bar` = shared::cluster address of CTA 0's mbarrier)
-__device__ __forceinline__ void tma2_load_2d_u32(uint32_t dst, uint64_t tmap, uint32_t bar, int c0, int c1) {
-    asm volatile(
-        "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-        ::"r"(dst), "l"(tmap), "r"(bar), "r"(c0), "r"(c1)
-        : "memory");
+// ---------------------------------------------------------------- wgmma
+// An MMA issued by a warpgroup reads its shared-memory operands asynchronously: fence before the first MMA that uses
+// register accumulators written by ordinary instructions, commit the issued MMAs as one group, and wait until at most
+// N groups are pending before their accumulators are read or their operand stage is handed back to the producer.
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() {
+    asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
 }
-__device__ __forceinline__ void tma2_load_4d_u32(uint32_t dst, uint64_t tmap, uint32_t bar, int c0, int c1, int c2, int c3) {
-    asm volatile(
-        "cp.async.bulk.tensor.4d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], "
-        "[%2];"
-        ::"r"(dst), "l"(tmap), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-        : "memory");
+// Keeps the compiler from moving accumulator reads / writes across an asynchronous MMA.
+template <int R>
+__device__ __forceinline__ void wgmma_fence_regs(float (&d)[R]) {
+#pragma unroll
+    for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
-__device__ __forceinline__ void umma2(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-__device__ __forceinline__ void umma2_commit_u32(uint32_t bar) {  // arrives on this barrier offset in BOTH CTAs
-    asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(bar),
-                 "h"((uint16_t)3)
-                 : "memory");
-}
-__device__ __forceinline__ void mbar_arrive_cta0(uint64_t* bar) {  // arrive on the same barrier offset in cluster CTA 0
-    asm volatile(
-        "{\n\t.reg .b32 ra;\n\t"
-        "mapa.shared::cluster.u32 ra, %0, 0;\n\t"
-        "mbarrier.arrive.release.cluster.shared::cluster.b64 _, [ra];\n\t}"
-        ::"r"(smem_u32(bar))
-        : "memory");
-}
-__device__ __forceinline__ uint32_t mapa_cta0(uint32_t saddr) {  // shared::cluster address of the same offset in CTA 0
-    uint32_t r;
-    asm volatile("mapa.shared::cluster.u32 %0, %1, 0;" : "=r"(r) : "r"(saddr));
-    return r;
-}
-
-
-// ---------------------------------------------------------------- tcgen05
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_dst, uint32_t ncols) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_dst)), "r"(ncols)
-                 : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish() {
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// D[tmem] (+)= A[smem] * B[smem], bf16 inputs, fp32 accumulate.  Issued by ONE thread.
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                          uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// Arrive on an mbarrier when all previously issued tcgen05.mma of this thread have completed.
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-                 : "memory");
-}
-
-// same, arriving on the barrier at this smem offset in every CTA of the cluster selected by cta_mask
-__device__ __forceinline__ void umma_commit_mcast(uint64_t* bar, uint16_t cta_mask) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-                     smem_u32(bar)),
-                 "h"(cta_mask)
-                 : "memory");
-}
-
-// 32 lanes x 32 consecutive fp32 columns: thread i of the warp receives row (lane base + i), columns [col, col+32)
-__device__ __forceinline__ void tmem_ld_32x32(uint32_t taddr, uint32_t (&v)[32]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-          "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]),
-          "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]),
-          "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-        : "r"(taddr)
-        : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
 
 // ---------------------------------------------------------------- descriptors
-// Shared-memory matrix descriptor (PTX ISA tcgen05 "matrix descriptor"):
-//   [0,14) start address >> 4 | [16,30) leading byte offset >> 4 | [32,46) stride byte offset >> 4
-//   [46,48) version = 1 (sm_100) | [49,52) base offset | [61,64) swizzle: 2 = 128B
-// K-major SW128 tile  [rows][64 bf16 = 128 B]: 8-row groups are 1024 B apart (SBO); LBO unused (=1).
-// MN-major SW128 tile [k rows][64 bf16 = 128 B] per 64-wide MN chunk: SBO = 1024 B between 8-k-row
-//   groups, LBO = byte distance between consecutive 64-element MN chunks.
-__device__ __forceinline__ uint64_t make_smem_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
+// Shared-memory matrix descriptor of wgmma (PTX ISA "matrix descriptor format"):
+//   [0,14) start address >> 4 | [16,30) leading byte offset >> 4 | [32,46) stride byte offset >> 4 | [62,64) swizzle: 1 = 128B
+// K-major SW128 tile  [rows][64 16-bit = 128 B]: 8-row groups are 1024 B apart (SBO); LBO unused (=1).  A 16-wide k-step
+//   advances the start address by 32 B (+2 in the descriptor).
+// MN-major SW128 tile [k rows][64 16-bit = 128 B] per 64-wide MN chunk: SBO = 1024 B between 8-k-row groups, LBO = byte
+//   distance between consecutive 64-element MN chunks.  A 16-deep k-step advances by 16 rows = 2048 B (+128).
+__device__ __forceinline__ uint64_t make_wgmma_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
     uint64_t d = 0;
     d |= (uint64_t)((saddr >> 4) & 0x3FFF);
     d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
     d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
-    d |= (uint64_t)1 << 46;
-    d |= (uint64_t)2 << 61;
+    d |= (uint64_t)1 << 62;
     return d;
 }
-// The instruction descriptor (make_idesc) follows the storage-format section below: its operand format bits depend on it.
 
 // ---------------------------------------------------------------- 16-bit storage format of the (hi, lo) planes
 // GDRN_STORE_F16 = 0: hi = bf16(x),  lo = bf16(x - hi)               (8 + 8 bits; fp32 exponent range)
@@ -260,12 +162,11 @@ __device__ __forceinline__ uint64_t make_smem_desc(uint32_t saddr, uint32_t lbo_
 //     The scaled residual has the magnitude of x itself, so it needs no extra exponent range; the scale is divided
 //     out exactly in the GEMM epilogues (cross-term accumulator) and in load8().  Gradients are kept in range by a
 //     static loss scale applied by the engine (Engine.grad_scale), like AMP's GradScaler in the reference's configs.)
-// Both planes must share one format: tcgen05.mma kind::f16 rejects mixed bf16 x fp16 operands (illegal instruction).
+// Both planes must share one format: one wgmma multiplies operands of a single 16-bit type (wgmma.cuh).
 #ifndef GDRN_STORE_F16
 #define GDRN_STORE_F16 0
 #endif
 #if GDRN_STORE_F16
-constexpr int kOperandFmt = 0;  // instruction-descriptor a/b format: F16
 constexpr float kLoScale = 2048.f;
 constexpr float kLoInvScale = 1.f / 2048.f;
 __device__ __forceinline__ uint32_t pack_hi2(float a, float b) {  // a -> low half, b -> high half
@@ -277,7 +178,6 @@ __device__ __forceinline__ void unpack_hi2(uint32_t w, float& a, float& b) {
     asm("{\n\t.reg .b16 l, h;\n\tmov.b32 {l, h}, %2;\n\tcvt.f32.f16 %0, l;\n\tcvt.f32.f16 %1, h;\n\t}" : "=f"(a), "=f"(b) : "r"(w));
 }
 #else
-constexpr int kOperandFmt = 1;  // BF16
 constexpr float kLoScale = 1.f;
 constexpr float kLoInvScale = 1.f;
 __device__ __forceinline__ uint32_t pack_hi2(float a, float b) {
@@ -309,13 +209,6 @@ __device__ __forceinline__ void split1(float x, uint16_t& h, uint16_t& l) {
     split2(x, 0.f, hh, ll);
     h = (uint16_t)(hh & 0xffffu);
     l = (uint16_t)(ll & 0xffffu);
-}
-// Instruction descriptor, kind::f16 (PTX ISA "instruction descriptor" table): c_format F32 (1 << 4), a / b operand format at
-// bits 7 / 10 (0 = F16, 1 = BF16; both planes share kOperandFmt), a_major bit 15, b_major bit 16 (0 = K-major, 1 = MN-major),
-// N >> 3 at [17,23), M >> 4 at [24,29).
-__host__ __device__ constexpr uint32_t make_idesc(int M, int N, int a_mn_major, int b_mn_major) {
-    return (1u << 4) | ((uint32_t)kOperandFmt << 7) | ((uint32_t)kOperandFmt << 10) | ((uint32_t)a_mn_major << 15) |
-           ((uint32_t)b_mn_major << 16) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
 }
 
 }  // namespace gdrn

@@ -1,10 +1,10 @@
 """Stand-alone Patch-PnP: `ConvPnPNet.forward(coor_feat, region, extents)` of the reference
-(core/gdrn_modeling/models/conv_pnp_net.py:111-157) on the sm_100a kernels -- BASELINE.json configs[3]
+(core/gdrn_modeling/models/conv_pnp_net.py:111-157) on the sm_90a kernels -- BASELINE.json configs[3]
 ("64x64x(3+64) correspondence maps -> R|t, batch 512").
 
     [B, 3|5, 64, 64] xyz (+2-D coords)  +  [B, 64, 64, 64] region attention  (+ extents [B, 3])
         -> gdrn_pnp_pack_input   NCHW fp32 -> NHWC 16-bit planes, 67 | 69 valid of 128 channels, xyz de-normalised
-        -> 3 x (tcgen05 implicit-GEMM conv 3x3 s2 -> GroupNorm(32)+ReLU)        64 -> 32 -> 16 -> 8
+        -> 3 x (wgmma implicit-GEMM conv 3x3 s2 -> GroupNorm(32)+ReLU)        64 -> 32 -> 16 -> 8
         -> fc1 (8192 -> 1024, LeakyReLU 0.1) -> fc2 (1024 -> 256, LeakyReLU) -> fc_r | fc_t (one 9-column GEMM)
         -> rot [B, 6], t [B, 3]  (fp32)
 
@@ -76,7 +76,7 @@ class PatchPnP:
     @torch.no_grad()
     def __call__(self, coor_feat: torch.Tensor, region: torch.Tensor | None = None, extents: torch.Tensor | None = None):
         if not coor_feat.is_cuda:
-            raise RuntimeError("gdr_net_b200 Patch-PnP runs on CUDA (sm_100a) only; there is no CPU fallback")
+            raise RuntimeError("gdr_net_b200 Patch-PnP runs on CUDA (sm_90a) only; there is no CPU fallback")
         n = self.net
         coor_feat = coor_feat.float().contiguous()
         region = None if region is None else region.float().contiguous()

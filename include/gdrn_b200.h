@@ -1,4 +1,4 @@
-/* libgdrn_b200.so -- C ABI of the B200-native GDR-Net hot path.
+/* libgdrn_b200.so -- C ABI of the H100-native (sm_90a) GDR-Net hot path.
  *
  * Drop-in boundary (SURVEY.md 8b): the reference has no native code on this path -- every op below is
  * today an ATen / cuDNN / cuBLAS call issued by the `nn.Module`s cited per function.  The in-repo
@@ -12,7 +12,7 @@
  *     from gdrn_last_error(); nothing throws across the ABI; entry points are re-entrant;
  *   - activations are NHWC bf16 "planar pairs": a hi plane and an optional lo plane with
  *     value = hi + lo.  nsplit = 1: bf16 tensor-core math on the hi plane only (lo pointers NULL);
- *     nsplit = 3: fp32-faithful mode, three tcgen05 MMAs per k-step (hi*hi + hi*lo + lo*hi).
+ *     nsplit = 3: fp32-faithful mode, three wgmma MMAs per k-step (hi*hi + hi*lo + lo*hi).
  */
 #ifndef GDRN_B200_H
 #define GDRN_B200_H
@@ -30,14 +30,10 @@ long gdrn_launch_count(void); /* kernels launched by this library since load */
 int gdrn_abi_version(void);
 int gdrn_storage_format(void); /* 0: bf16 (hi, lo) planes; 1: fp16 planes, lo = fp16((x - hi) * gdrn_lo_scale()) */
 float gdrn_lo_scale(void);
-int gdrn_set_2cta(int on); /* A/B: cta_group::2 pair tiles (256x256 1-pass / 256x128 3-pass) for eligible conv layers; default on */
-long gdrn_2cta_launch_count(void); /* launches of the 2-CTA kernel since load */
 int gdrn_set_pdl(int on); /* A/B: programmatic dependent launch of the GEMM kernels (prologue under the predecessor's tail); default on, GDRN_PDL=0 disables */
-int gdrn_set_wgrad_2cta(int on); /* A/B: cta_group::2 pair tiles (256 co x 128/256 ci) for single-plane weight gradients with Cout % 256 == 0; default OFF (bit-equal to the 1-CTA kernel, no in-situ gain) */
-long gdrn_wgrad_2cta_launch_count(void);
-int gdrn_last_gemm_variant(void); /* BLOCK_N*10 + nsplit (+10000: 2-CTA kernel) of this thread's last conv/gemm forward launch */
+int gdrn_last_gemm_variant(void); /* BLOCK_N*10 + nsplit of this thread's last conv/gemm forward launch */
 
-/* ---- tcgen05 implicit-GEMM convolution, forward (and dgrad with flipped/transposed weights) ------------
+/* ---- wgmma implicit-GEMM convolution, forward (and dgrad with flipped/transposed weights) ------------
  * replaces nn.Conv2d / nn.ConvTranspose2d forward: resnet_backbone.py:21-49,69-76 (torchvision BasicBlock),
  * cdpn_rot_head_region.py:82-135, conv_pnp_net.py:76-80.
  * x [N,H,W,Cin] (Cin % 64 == 0), w packed [Cout_pad][KH*KW*Cin] (gdrn_pack_weight), outputs row-major

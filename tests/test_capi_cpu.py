@@ -1,4 +1,4 @@
-"""CPU: the C-ABI library builds for sm_100a, loads, and exports every symbol include/gdrn_b200.h declares
+"""CPU: the C-ABI library builds for sm_90a, loads, and exports every symbol include/gdrn_b200.h declares
 (no compute calls without a GPU)."""
 import ctypes
 import os
@@ -38,13 +38,13 @@ def test_argument_errors_do_not_need_a_gpu(dll):
     assert rc == -1 and b"K=" in dll.gdrn_last_error()
 
 
-def test_sass_has_tcgen05_and_tma():
-    """The shipped library contains Blackwell tensor-core / TMA instructions (UTCHMMA, UTMALDG, LDTM)."""
+def test_sass_has_wgmma_and_tma():
+    """The shipped library contains Hopper warpgroup tensor-core / TMA instructions (HGMMA, UTMALDG)."""
     import shutil
     import subprocess
 
     if shutil.which("cuobjdump") is None:
         pytest.skip("cuobjdump not available")
     sass = subprocess.run(["cuobjdump", "-sass", capi.LIB_PATH], capture_output=True, text=True).stdout
-    for mnem in ("UTCHMMA", "UTMALDG", "LDTM"):
+    for mnem in ("HGMMA", "UTMALDG"):
         assert mnem in sass, mnem

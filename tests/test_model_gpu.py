@@ -3,7 +3,7 @@
   (b) the CPU oracle (oracle/gdrn_oracle.py) on the same seeded inputs.
 
 Tolerances (BASELINE.json north_star): outputs within 1e-3 relative fp32, region argmax bit-exact -- asserted in
-the fp32-faithful "fp32x3" mode (three tcgen05 passes over hi/lo fp16 planes = 22-bit operands).  The single-pass
+the fp32-faithful "fp32x3" mode (three wgmma passes over hi/lo fp16 planes = 22-bit operands).  The single-pass
 "half" mode (fp16 operands: 11-bit mantissa, the same as the TF32 convolutions cuDNN runs for the reference) is the
 throughput mode; its deviation is bounded by operand rounding (2^-12 per tensor per layer, accumulating over ~130
 roundings) and is asserted at the looser, documented bound below.

@@ -104,42 +104,6 @@ def test_conv_fwd(planes, case):
         assert _rel(stats[1], s2) < 1e-4
 
 
-@pytest.mark.parametrize("planes,case", [(1, (8, 64, 256, 256, 1)), (2, (8, 64, 256, 256, 1)), (1, (16, 32, 128, 256, 1)),
-                                         (2, (16, 32, 128, 128, 1)), (2, (16, 64, 64, 128, 2)), (1, (64, 32, 256, 512, 2)),
-                                         (1, (16, 32, 128, 128, 1))])  # last: the 256 x 128 one-pass pair tile
-def test_conv_fwd_2cta_variant(planes, case):
-    """The cta_group::2 kernel (one 256 x 256 [1 pass] / 256 x 128 [3 pass] tile per CTA pair) on layers that select it,
-    against the 1-CTA kernel's reference AND bit-compared with the 1-CTA kernel itself (same MMAs, same accumulation order)."""
-    ops = _ops()
-    from gdr_net_b200.capi import C
-
-    dll = C.load()
-    N, H, Cin, Cout, stride = case
-    g = torch.Generator(device="cuda").manual_seed(77 + sum(case))
-    x = torch.randn(N, Cin, H, H, device="cuda", generator=g)
-    w = torch.randn(Cout, Cin, 3, 3, device="cuda", generator=g) / math.sqrt(9 * Cin)
-    X, Wp = _nhwc(x, planes), ops.pack_conv_fwd(w, planes)
-    Ho = H // stride
-    outs = []
-    try:
-        for mode in (1, 0):
-            C.gdrn_set_2cta(mode)
-            out32 = torch.zeros(N, Ho, Ho, Cout, device="cuda")
-            stats = torch.zeros(2, Cout, device="cuda")
-            n0 = dll.gdrn_2cta_launch_count()
-            Y = ops.conv_fwd(X, Wp, Cout, 3, 3, stride, 1, out_f32=out32, stats=stats)
-            torch.cuda.synchronize()
-            if mode == 1:
-                assert dll.gdrn_2cta_launch_count() == n0 + 1, "the shape did not select the 2-CTA kernel"
-            outs.append((out32, stats, Y.float()))
-    finally:
-        C.gdrn_set_2cta(1)
-    ref = F.conv2d(_operand(x, planes), _operand(w, planes), None, stride=stride, padding=1).permute(0, 2, 3, 1)
-    assert _rel(outs[0][0], ref) < TOL[planes]
-    assert _rel(outs[0][1][1], (ref.reshape(-1, Cout) ** 2).sum(0)) < 1e-4
-    assert torch.equal(outs[0][0], outs[1][0]) and torch.equal(outs[0][2], outs[1][2])  # identical arithmetic in both kernels
-
-
 @pytest.mark.parametrize("planes", [1, 2])
 def test_conv_dgrad_as_conv(planes):
     """dX of a 3x3 s1 conv = conv(dY, flipped/transposed weights); of a s2 conv = same over zero-inserted dY."""
@@ -260,42 +224,6 @@ def test_conv_wgrad(planes, case):
     ops.unpack_wgrad(buf, grad, Cout, Cin, k, k, Cin, ks, ks_stride, Cin * k * k, k * k, k, 1)
     torch.cuda.synchronize()
     assert _rel(grad, gw) < 5e-5
-
-
-@pytest.mark.parametrize("case", [(4, 16, 16, 256, 256, 3, 1, 1), (8, 8, 8, 512, 512, 3, 1, 1), (2, 32, 32, 128, 256, 3, 2, 1),
-                                  (2, 32, 32, 128, 256, 1, 2, 0), (64, 8, 8, 512, 512, 3, 1, 1), (8, 32, 32, 256, 256, 3, 1, 1),
-                                  (3, 16, 16, 256, 512, 3, 2, 1)])
-def test_conv_wgrad_2cta_variant(case):
-    """Single-plane weight gradient on CTA pairs (256 co x 128/256 ci per pair) against autograd AND bit-compared with the
-    1-CTA kernel (same MMAs per accumulator, same k order, same split-K partition)."""
-    ops = _ops()
-    from gdr_net_b200.capi import C
-
-    dll = C.load()
-    N, H, W, Cin, Cout, k, stride, pad = case
-    g = torch.Generator(device="cuda").manual_seed(sum(case) + 5)
-    x = torch.randn(N, Cin, H, W, device="cuda", generator=g)
-    w = torch.zeros(Cout, Cin, k, k, device="cuda", requires_grad=True)
-    y = F.conv2d(_operand(x, 1), w, None, stride=stride, padding=pad)
-    dy = torch.randn_like(y) / 8
-    (gw,) = torch.autograd.grad(y, w, _operand(dy, 1))
-    grads = []
-    try:
-        for mode in (1, 0):
-            C.gdrn_set_wgrad_2cta(mode)
-            ws = ops.Workspace()
-            n0 = dll.gdrn_wgrad_2cta_launch_count()
-            buf, ks, ks_stride = ops.conv_wgrad(_nhwc(dy, 1), _nhwc(x, 1), ws, Cout, k, k, stride, pad)
-            grad = torch.zeros_like(w)
-            ops.unpack_wgrad(buf, grad, Cout, Cin, k, k, Cin, ks, ks_stride, Cin * k * k, k * k, k, 1)
-            torch.cuda.synchronize()
-            if mode == 1:
-                assert dll.gdrn_wgrad_2cta_launch_count() == n0 + 1, "the shape did not select the pair kernel"
-            grads.append(grad)
-    finally:
-        C.gdrn_set_wgrad_2cta(0)  # the library default (the pair kernel is neutral-to-slower inside the step)
-    assert _rel(grads[0], gw) < 5e-5
-    assert torch.equal(grads[0], grads[1])
 
 
 @pytest.mark.parametrize("planes", [1, 2])

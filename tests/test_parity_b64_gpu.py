@@ -123,7 +123,7 @@ def test_mixed_gradients_b4_vs_oracle():
         out[precision] = (worst, med, cos, {k: float(v) for k, v in loss_dict.items()})
     for k, v in out["mixed"][3].items():  # the forward IS the fp32x3 forward
         assert abs(v - float(o["losses"][k])) <= REL * abs(float(o["losses"][k])), k
-    # measured (r2, B200): fp32x3 worst 0.040 / median 2.5e-2 / cosine 0.99967; mixed worst 0.035 / median 2.7e-2 / cosine 0.99960
+    # measured (H100 80GB HBM3, 400 W): fp32x3 worst 0.032 / median 2.4e-2 / cosine 0.99967; mixed worst 0.035 / median 2.6e-2 / cosine 0.99963
     # -- the single-pass backward adds nothing visible on top of the non-smooth forward's own noise floor
     assert out["mixed"][0][1] < 0.06 and out["mixed"][2] > 0.999, out["mixed"][:3]
     # medians move between runs (1.8e-2 .. 2.7e-2 seen for BOTH modes: atomics reorder sums, borderline ReLU / L1 decisions flip),
@@ -325,7 +325,7 @@ def test_eval_folded_bn_matches_unfused_and_oracle():
 def test_deterministic_mode_is_bit_reproducible_and_graph_equals_eager():
     """Engine.deterministic: BatchNorm batch statistics and backward sums use two-stage ordered reductions (no atomics), so a
     step is bit-identical run to run -- which turns the graph-replay and gradient-accumulation checks into EXACT comparisons
-    (the default path's fp32 atomics give ~1e-7 jitter that the non-smooth network amplifies to 1e-2 on backbone gradients)."""
+    (the epilogue-atomics path's fp32 atomics give ~1e-7 jitter that the non-smooth network amplifies to 1e-2 on backbone gradients)."""
     from oracle import fixtures
 
     sd = fixtures.calibrated_state_dict(0)
@@ -351,9 +351,10 @@ def test_deterministic_mode_is_bit_reproducible_and_graph_equals_eager():
             assert other[0][k] == runs[0][0][k], (k, other[0][k], runs[0][0][k])
         for n in exact:
             assert torch.equal(other[1][n], runs[0][1][n]), n
-    # and the deterministic statistics agree with the default (epilogue-atomics) path to fp32 rounding
+    # and the deterministic statistics agree with the epilogue-atomics path to fp32 rounding
     model = _build("mixed", sd)
     model.train()
+    model.engine.deterministic = False
     _, ld = model(batch["roi_img"], **synth.forward_kwargs(batch, train=True))
     for k, v in ld.items():
         assert abs(float(v) - runs[0][0][k]) <= 2e-5 * abs(runs[0][0][k]) + 1e-7, k

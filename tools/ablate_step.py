@@ -1,6 +1,6 @@
 """In-situ cost of each non-GEMM kernel family inside the graphed train step (runs on the GPU box).
 
-ncu's per-launch durations are cold-cache and serialised; producer/consumer pairs that live in the 126 MB L2 (split-K
+ncu's per-launch durations are cold-cache and serialised; producer/consumer pairs that live in the 50 MB L2 (split-K
 workspace -> unpack, conv output -> BN) look 2-5x more expensive there than they are inside the step.  Here each family's
 C entry point is replaced by a no-op, the whole step is re-captured as a CUDA graph and re-timed: baseline - ablated = the
 family's real share.  (The ablated step computes garbage; only its duration is used.)

@@ -1,4 +1,4 @@
-"""Micro-benchmark of the tcgen05 conv kernels on the GDR-Net layer shapes (B=64), CUDA-event timed."""
+"""Micro-benchmark of the wgmma conv kernels on the GDR-Net layer shapes (B=64), CUDA-event timed."""
 import json
 import sys
 import os

@@ -1,4 +1,4 @@
-"""Experiment: fp32 accumulation behaviour of tcgen05.mma (bias / growth with K) vs fp64 truth."""
+"""Experiment: fp32 accumulation behaviour of the GEMM kernels' tensor-core MMAs (bias / growth with K) vs fp64 truth."""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch

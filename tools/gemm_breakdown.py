@@ -1,4 +1,4 @@
-"""Per-launch timing of every tcgen05 GEMM/conv launch in one B=64 train step (CUDA events), with algorithmic TFLOP/s."""
+"""Per-launch timing of every wgmma GEMM/conv launch in one B=64 train step (CUDA events), with algorithmic TFLOP/s."""
 import os, sys, json
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
