@@ -1,5 +1,5 @@
 // Tile epilogue of the implicit-GEMM forward kernel (gemm_fwd.cu), run by each MMA warpgroup on its 64 x BLOCK_N register
-// accumulators: (+ cross-term accumulator of the 3-pass mode) -> bias -> residual -> activation -> 16-bit hi[/lo] and / or fp32
+// accumulators: bias -> residual -> activation -> 16-bit hi[/lo] and / or fp32
 // stores -> per-channel sum / sum of squares for the BatchNorm batch statistics.
 #pragma once
 #include "gdrn_internal.h"
@@ -8,32 +8,38 @@
 
 namespace gdrn {
 
-// acc    : this thread's accumulator fragment (wgmma.cuh layout), BLOCK_N / 2 main values followed, in the 3-pass mode, by
-//          BLOCK_N / 2 cross-term values (scaled by the lo-plane scale);
+// acc    : this thread's BLOCK_N / 2 accumulator values (wgmma.cuh layout; in the 3-pass mode the cross terms are already folded in);
 // row0   : row of the 128-row tile held in acc[4j + 0..1] (acc[4j + 2..3] hold row0 + 8); q = lane % 4 selects the column pair;
 // s_stats: the CTA's [2][BLOCK_N] partial BatchNorm sums.
 // Columns are written in 32-wide chunks like the output tiles: a chunk that starts at or beyond N is left untouched, inside a
 // partial chunk the columns in [N, ldc) are zero-filled.
-template <int BLOCK_N, int NSPLIT>
+// The only per-row state kept across the unrolled column loop is one 32-bit element offset (and a validity flag) per row,
+// shared by the output and residual planes; the host entry points reject outputs with rows * ldc >= 2^32.  Addresses are
+// rebuilt from the kernel parameters for every chunk: unsigned arithmetic keeps the compiler from hoisting them into 64-bit
+// per-row pointers, which would not fit next to the accumulators of a 128-wide 3-pass tile.
+template <int BLOCK_N>
 __device__ __forceinline__ void gemm_epilogue_tile(const GemmParams& p, const float* acc, int lane, int row0, int m_tile, int n_tile,
                                                    int ph, float* s_stats) {
     __nv_bfloat16* out_hi = reinterpret_cast<__nv_bfloat16*>(p.out_hi);
     __nv_bfloat16* out_lo = reinterpret_cast<__nv_bfloat16*>(p.out_lo);
+    const __nv_bfloat16* res_hi = reinterpret_cast<const __nv_bfloat16*>(p.res_hi);
+    const __nv_bfloat16* res_lo = reinterpret_cast<const __nv_bfloat16*>(p.res_lo);
     const int q = lane & 3;
-    long grow[2];
+    uint32_t off[2];  // element offset of (output row, this thread's first column) in the [rows][ldc] planes
     bool row_ok[2];
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
-        const long mrow = (long)m_tile * 128 + row0 + 8 * h;
+        const int mrow = m_tile * 128 + row0 + 8 * h;
         row_ok[h] = mrow < p.M;
-        grow[h] = mrow;  // output row
+        uint32_t grow = (uint32_t)mrow;  // output row
         if (p.nphase) {  // (n, i, j) of the dY lattice -> pixel (2i + a, 2j + b) of the 2x larger dX
-            const long j = mrow & ((1L << p.pw_log2) - 1);
-            const long t = mrow >> p.pw_log2;
-            const long i = t & ((1L << p.ph_log2) - 1);
-            const long n = t >> p.ph_log2;
-            grow[h] = (((n << (p.ph_log2 + 1)) + 2 * i + p.ph_a[ph]) << (p.pw_log2 + 1)) + 2 * j + p.ph_b[ph];
+            const uint32_t j = grow & ((1u << p.pw_log2) - 1);
+            const uint32_t t = grow >> p.pw_log2;
+            const uint32_t i = t & ((1u << p.ph_log2) - 1);
+            const uint32_t n = t >> p.ph_log2;
+            grow = (((n << (p.ph_log2 + 1)) + 2 * i + p.ph_a[ph]) << (p.pw_log2 + 1)) + 2 * j + p.ph_b[ph];
         }
+        off[h] = grow * (uint32_t)p.ldc + (uint32_t)(n_tile * BLOCK_N + 2 * q);
     }
 #pragma unroll
     for (int j = 0; j < BLOCK_N / 8; ++j) {
@@ -45,10 +51,7 @@ __device__ __forceinline__ void gemm_epilogue_tile(const GemmParams& p, const fl
 #pragma unroll
         for (int h = 0; h < 2; ++h)
 #pragma unroll
-            for (int e = 0; e < 2; ++e) {
-                f[h][e] = acc[4 * j + 2 * h + e];
-                if (NSPLIT == 3) f[h][e] = fmaf(acc[BLOCK_N / 2 + 4 * j + 2 * h + e], kLoInvScale, f[h][e]);
-            }
+            for (int e = 0; e < 2; ++e) f[h][e] = acc[4 * j + 2 * h + e];
         if (p.bias != nullptr) {
             const float b0 = ok0 ? __ldg(p.bias + col) : 0.f, b1 = ok1 ? __ldg(p.bias + col + 1) : 0.f;
 #pragma unroll
@@ -57,17 +60,17 @@ __device__ __forceinline__ void gemm_epilogue_tile(const GemmParams& p, const fl
                 f[h][1] += b1;
             }
         }
-        if (p.res_hi != nullptr && ok0) {
+        if (res_hi != nullptr && ok0) {
             // folded eval epilogue: + residual (the block's identity / downsample branch, same [rows][ldc] planes; N % 32 == 0)
 #pragma unroll
             for (int h = 0; h < 2; ++h) {
                 if (!row_ok[h]) continue;
                 float a, b;
-                unpack_hi2(__ldg(reinterpret_cast<const uint32_t*>(reinterpret_cast<const __nv_bfloat16*>(p.res_hi) + grow[h] * p.ldc + col)), a, b);
+                unpack_hi2(__ldg(reinterpret_cast<const uint32_t*>(res_hi + (off[h] + 8 * j))), a, b);
                 f[h][0] += a;
                 f[h][1] += b;
-                if (p.res_lo != nullptr) {
-                    unpack_lo2(__ldg(reinterpret_cast<const uint32_t*>(reinterpret_cast<const __nv_bfloat16*>(p.res_lo) + grow[h] * p.ldc + col)), a, b);
+                if (res_lo != nullptr) {
+                    unpack_lo2(__ldg(reinterpret_cast<const uint32_t*>(res_lo + (off[h] + 8 * j))), a, b);
                     f[h][0] += a;
                     f[h][1] += b;
                 }
@@ -85,16 +88,17 @@ __device__ __forceinline__ void gemm_epilogue_tile(const GemmParams& p, const fl
             for (int h = 0; h < 2; ++h) {
                 if (!row_ok[h]) continue;
                 const float a = ok0 ? f[h][0] : 0.f, b = ok1 ? f[h][1] : 0.f;
-                if (p.out_f32 != nullptr) *reinterpret_cast<float2*>(p.out_f32 + grow[h] * p.ldc + col) = make_float2(a, b);
+                const uint32_t o = off[h] + 8 * j;
+                if (p.out_f32 != nullptr) *reinterpret_cast<float2*>(p.out_f32 + o) = make_float2(a, b);
                 if (out_hi != nullptr) {
                     uint32_t hi, lo;
                     if (out_lo != nullptr) {
                         split2(a, b, hi, lo);
-                        *reinterpret_cast<uint32_t*>(out_lo + grow[h] * p.ldc + col) = lo;
+                        *reinterpret_cast<uint32_t*>(out_lo + o) = lo;
                     } else {
                         hi = pack_hi2(a, b);
                     }
-                    *reinterpret_cast<uint32_t*>(out_hi + grow[h] * p.ldc + col) = hi;
+                    *reinterpret_cast<uint32_t*>(out_hi + o) = hi;
                 }
             }
         }

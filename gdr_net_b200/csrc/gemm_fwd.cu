@@ -18,9 +18,11 @@
 //     stores 16-bit hi[/lo] or fp32 and accumulates the per-channel BatchNorm statistics).  While the MMA
 //     warpgroups run a tile's epilogue the producer already fills the stages of the next tile.
 //     Warp 8 = TMA producer.  With nine warps ptxas allots at most 168 registers per thread (three warps share one SM
-//     sub-partition's register file).  Tiles are 128 wide in one pass (64 accumulator registers) and 64 wide in three
-//     passes (main + cross accumulators, 64 registers): a 128-wide 3-pass tile needs 128 accumulator registers and, with
-//     the epilogue's row / residual / output state, spills under that limit (ptxas -v: 152 bytes).
+//     sub-partition's register file).  A 128-wide 3-pass tile holds 128 accumulator registers (main + cross) in its main
+//     loop; it fits (ptxas -v: 162 registers, no spills) because the cross accumulator is folded into the main one before
+//     the epilogue and the epilogue keeps only a 32-bit element offset per row live.  The width matters for the 3-pass mode: per
+//     MMA clock a k-block moves about 190 B of shared memory (wgmma operand reads + TMA writes) at 128 x 64 and about 135 B at
+//     128 x 128, against 128 B/clk per SM, so the 64-wide 3-pass tile is bound by shared-memory bandwidth.
 //   * NSPLIT = 3 is the fp32-faithful mode: operands are (hi, lo) 16-bit planes and each k-step issues
 //     hi*hi + hi*lo + lo*hi (the lo*lo term, 2^-22 relative with fp16 planes, is dropped).
 #include <stdlib.h>
@@ -49,7 +51,7 @@ struct GemmCfg {
     static constexpr int STAGES = STAGES_RAW > 8 ? 8 : STAGES_RAW;
     static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + kAuxBytes + 1024;
     // 3-pass mode: the small cross terms (hi*lo + lo*hi) are kept in their own accumulator and added to the main one with a
-    // round-to-nearest fp32 fma in the epilogue.  Each k-step issues three MMAs of width BLOCK_N, each writing one WHOLE
+    // round-to-nearest fp32 fma before the epilogue.  Each k-step issues three MMAs of width BLOCK_N, each writing one WHOLE
     // accumulator: a_hi x [w_hi; w_lo] as one 2 * BLOCK_N-wide MMA followed by a_lo x w_hi into its upper half would read
     // a_hi once less, but an MMA that writes part of the registers of one still in flight makes ptxas serialise the whole
     // wgmma chain (warning C7511); the three-MMA form measured 0.9 % faster per step.
@@ -242,7 +244,16 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_fwd_kernel(const __grid_cons
         wgmma_wait<0>();
         wgmma_fence_regs(acc);
         if (prev_stage >= 0 && signaller) mbar_arrive(&empty_bar[prev_stage]);
-        gemm_epilogue_tile<BLOCK_N, NSPLIT>(p, acc, lane, cw * 64 + (warp & 3) * 16 + (lane >> 2), m_tile, n_tile, ph, s_stats);
+        if constexpr (NSPLIT == 3) {
+            // fold the cross terms into the main accumulator before the epilogue; the empty asm pins each sum here, so the
+            // cross registers are dead before the epilogue's address and output work starts
+#pragma unroll
+            for (int i = 0; i < BLOCK_N / 2; ++i) {
+                acc[i] = fmaf(acc[BLOCK_N / 2 + i], kLoInvScale, acc[i]);
+                asm volatile("" : "+f"(acc[i]));
+            }
+        }
+        gemm_epilogue_tile<BLOCK_N>(p, acc, lane, cw * 64 + (warp & 3) * 16 + (lane >> 2), m_tile, n_tile, ph, s_stats);
     }
     if (p.stats != nullptr) {
         asm volatile("bar.sync 1, 256;" ::: "memory");  // the two MMA warpgroups only
@@ -301,6 +312,7 @@ static int dispatch_gemm(const GemmParams& p, int block_n, int nsplit, cudaStrea
         if (block_n == 128) return launch_gemm<128, 1>(p, stream);
         if (block_n == 64) return launch_gemm<64, 1>(p, stream);
     } else if (nsplit == 3) {
+        if (block_n == 128) return launch_gemm<128, 3>(p, stream);
         if (block_n == 64) return launch_gemm<64, 3>(p, stream);
     }
     return set_error(GDRN_ERR_ARG, "gemm: unsupported block_n=%d nsplit=%d", block_n, nsplit);
@@ -308,9 +320,8 @@ static int dispatch_gemm(const GemmParams& p, int block_n, int nsplit, cudaStrea
 
 // Tile width: the widest BLOCK_N (fewest A re-reads, best smem-bandwidth ratio) that still yields >= ~0.75 waves of
 // CTAs on the SMs; small-M layers (layer4, FC) fall back to narrower tiles instead of leaving SMs idle.
-static int pick_block_n(int n_pad, int nsplit, int num_m_tiles) {
+static int pick_block_n(int n_pad, int num_m_tiles) {
     if (n_pad % 64 != 0) return -1;
-    if (nsplit == 3) return 64;  // the widest 3-pass tile that does not spill (see the header comment)
     if (n_pad % 128 == 0 && num_m_tiles * (n_pad / 128) >= (num_sms() * 3) / 4) return 128;
     if (num_m_tiles * (n_pad / 128) < num_sms() / 2) return 64;
     return n_pad % 128 == 0 ? 128 : 64;
@@ -336,11 +347,12 @@ extern "C" int gdrn_conv_fwd(const void* x_hi, const void* x_lo, const void* w_h
     if (act < 0 || act > 2) return set_error(GDRN_ERR_ARG, "conv_fwd: act must be 0 (none), 1 (LeakyReLU 0.1) or 2 (ReLU)");
     const int Ho = H / stride, Wo = W / stride;
     if (Wo > 128 || 128 % Wo != 0) return set_error(GDRN_ERR_ARG, "conv_fwd: unsupported output width %d", Wo);
+    if ((uint64_t)N * Ho * Wo * ldc > UINT32_MAX) return set_error(GDRN_ERR_ARG, "conv_fwd: output too large for 32-bit offsets");
     int TH = 128 / Wo;
     if (TH > Ho) TH = Ho;
     const int TN = 128 / (Wo * TH);
     if (Ho % TH != 0) return set_error(GDRN_ERR_ARG, "conv_fwd: Ho=%d not divisible by tile rows %d", Ho, TH);
-    const int block_n = pick_block_n(Cout_pad, nsplit, (N * Ho * Wo + 127) / 128);
+    const int block_n = pick_block_n(Cout_pad, (N * Ho * Wo + 127) / 128);
     if (block_n < 0) return set_error(GDRN_ERR_ARG, "conv_fwd: Cout_pad=%d must be a multiple of 64", Cout_pad);
 
     GemmParams p;
@@ -405,13 +417,14 @@ extern "C" int gdrn_conv_dgrad_s2(const void* du_hi, const void* du_lo, const vo
     if (Cy % 64 != 0) return set_error(GDRN_ERR_ARG, "conv_dgrad_s2: Cy=%d must be a multiple of 64", Cy);
     if (ldc % 8 != 0 || ldc < Cx) return set_error(GDRN_ERR_ARG, "conv_dgrad_s2: bad ldc=%d", ldc);
     if (Wo > 128 || 128 % Wo != 0 || (Ho & (Ho - 1)) != 0) return set_error(GDRN_ERR_ARG, "conv_dgrad_s2: unsupported dY size %dx%d", Ho, Wo);
+    if ((uint64_t)N * 4 * Ho * Wo * ldc > UINT32_MAX) return set_error(GDRN_ERR_ARG, "conv_dgrad_s2: output too large for 32-bit offsets");
     int TH = 128 / Wo;
     if (TH > Ho) TH = Ho;
     const int TN = 128 / (Wo * TH);
     if (Ho % TH != 0) return set_error(GDRN_ERR_ARG, "conv_dgrad_s2: Ho=%d not divisible by tile rows %d", Ho, TH);
     const int num_m_tiles = (N * Ho * Wo + 127) / 128;
     const int nphase = K == 3 ? 4 : 1;
-    const int block_n = pick_block_n(Cx_pad, nsplit, num_m_tiles * nphase);
+    const int block_n = pick_block_n(Cx_pad, num_m_tiles * nphase);
     if (block_n < 0) return set_error(GDRN_ERR_ARG, "conv_dgrad_s2: Cx_pad=%d must be a multiple of 64", Cx_pad);
 
     GemmParams p;
@@ -483,7 +496,8 @@ extern "C" int gdrn_gemm_fwd(const void* a_hi, const void* a_lo, const void* w_h
     if (nsplit == 3 && (a_lo == nullptr || w_lo == nullptr)) return set_error(GDRN_ERR_ARG, "gemm_fwd: lo planes missing");
     if (K % 64 != 0) return set_error(GDRN_ERR_ARG, "gemm_fwd: K=%d must be a multiple of 64", K);
     if (ldc % 8 != 0 || ldc < N) return set_error(GDRN_ERR_ARG, "gemm_fwd: bad ldc=%d", ldc);
-    const int block_n = pick_block_n(N_pad, nsplit, (M + 127) / 128);
+    if ((uint64_t)M * ldc > UINT32_MAX) return set_error(GDRN_ERR_ARG, "gemm_fwd: output too large for 32-bit offsets");
+    const int block_n = pick_block_n(N_pad, (M + 127) / 128);
     if (block_n < 0) return set_error(GDRN_ERR_ARG, "gemm_fwd: N_pad=%d must be a multiple of 64", N_pad);
     GemmParams p;
     memset(&p, 0, sizeof(p));
