@@ -853,8 +853,305 @@ __global__ void __launch_bounds__(kPnpThreads) pnp_final_kernel(const double* __
     }
 }
 
+// ------------------------------------------------------------------------------------------------ network-initialised iterative PnP
+// cv2.solvePnP(SOLVEPNP_ITERATIVE, useExtrinsicGuess=True) of the evaluator's net_iter_pnp mode (gdrn_evaluator.py:187-314):
+// OpenCV's cvFindExtrinsicCameraParams2 with a guess = Levenberg-Marquardt (CvLevMarq) on p = (rvec, tvec), residual = projected
+// pixel - image point.  oracle/net_pnp_oracle.py restates it (pinned against cv2: 1e-9) and this kernel follows that restatement:
+//   CALC_J    J, r at p -> JtJ, Jtr (one block reduction of 28 sums); prev = p; p = prev - solve(JtJ, diag * (1 + 10^l), Jtr)
+//             by SVD; the first time prevErr = |r|
+//   CHECK_ERR err = |r(p)|; err > prevErr and ++l <= 16: re-solve from prev, check again; else l = max(l - 1, -16), ++iters,
+//             stop at iters >= max_iters or |p - prev| / (|prev| + DBL_EPSILON) < FLT_EPSILON, else prevErr = err -> CALC_J
+// The serial part (6x6 solve, state machine, Rodrigues both ways) runs on thread 0 with its scratch in shared memory.
+struct LmShared {
+    double p[6], prev[6];
+    double JtJ[36], Jtr[6];
+    double At[36], Vt[36], w[6];  // SVD scratch (6x6 solve; the 3x3 re-orthonormalisation uses the leading 9 entries)
+    double R[9], dRdr[27];        // R(p[0:3]) and dR / dr (row j = derivative by r_j of the 9 entries of R, row-major)
+    double prev_err;
+    int lam, iters, phase;  // phase: 0 = check the error again, 1 = new Jacobian, 2 = done
+};
+
+// cv::Rodrigues, vector -> matrix, with the 3x9 derivative
+__device__ void rodrigues_v2m(const double* r, double* R, double* J) {
+    const double theta = sqrt(r[0] * r[0] + r[1] * r[1] + r[2] * r[2]);
+    if (theta < 2.220446049250313e-16) {
+        for (int k = 0; k < 9; ++k) R[k] = (k % 4 == 0) ? 1.0 : 0.0;
+        for (int k = 0; k < 27; ++k) J[k] = 0.0;
+        J[5] = -1;
+        J[7] = 1;
+        J[9 + 2] = 1;
+        J[9 + 6] = -1;
+        J[18 + 1] = -1;
+        J[18 + 3] = 1;
+        return;
+    }
+    const double c = cos(theta), s = sin(theta), c1 = 1.0 - c, itheta = 1.0 / theta;
+    const double rx = r[0] * itheta, ry = r[1] * itheta, rz = r[2] * itheta;
+    const double rrt[9] = {rx * rx, rx * ry, rx * rz, rx * ry, ry * ry, ry * rz, rx * rz, ry * rz, rz * rz};
+    const double r_x[9] = {0, -rz, ry, rz, 0, -rx, -ry, rx, 0};
+    const double I[9] = {1, 0, 0, 0, 1, 0, 0, 0, 1};
+    for (int k = 0; k < 9; ++k) R[k] = c * I[k] + c1 * rrt[k] + s * r_x[k];
+    const double drrt[27] = {rx + rx, ry, rz, ry, 0, 0, rz, 0, 0, 0, rx, 0, rx, ry + ry, rz, 0, rz, 0, 0, 0, rx, 0, 0, ry, rx, ry, rz + rz};
+    const double d_r_x[27] = {0, 0, 0, 0, 0, -1, 0, 1, 0, 0, 0, 1, 0, 0, 0, -1, 0, 0, 0, -1, 0, 1, 0, 0, 0, 0, 0};
+    for (int i = 0; i < 3; ++i) {
+        const double ri = i == 0 ? rx : i == 1 ? ry : rz;
+        const double a0 = -s * ri, a1 = (s - 2 * c1 * itheta) * ri, a2 = c1 * itheta, a3 = (c - s * itheta) * ri, a4 = s * itheta;
+        for (int k = 0; k < 9; ++k) J[i * 9 + k] = a0 * I[k] + a1 * rrt[k] + a2 * drrt[i * 9 + k] + a3 * r_x[k] + a4 * d_r_x[i * 9 + k];
+    }
+}
+
+// cv::Rodrigues, matrix -> vector: SVD re-orthonormalisation (R = U V^T), then the axis / angle closed forms with OpenCV's
+// theta ~ 0 and theta ~ pi branches.  `at`, `vt`, `w` are 9 / 9 / 3 doubles of scratch.
+__device__ void rodrigues_m2v(const double* Rin, double* r, double* at, double* vt, double* w) {
+    for (int j = 0; j < 3; ++j)
+        for (int k = 0; k < 3; ++k) at[3 * k + j] = Rin[3 * j + k];  // rows of `at` = columns of R
+    jacobi_svd(at, 3, w, vt, 3, 3, 3);
+    double R[9];
+    for (int i = 0; i < 3; ++i)
+        for (int j = 0; j < 3; ++j) R[3 * i + j] = at[0 + i] * vt[0 + j] + at[3 + i] * vt[3 + j] + at[6 + i] * vt[6 + j];
+    double rx = R[7] - R[5], ry = R[2] - R[6], rz = R[3] - R[1];
+    const double s = sqrt((rx * rx + ry * ry + rz * rz) * 0.25);
+    double c = (R[0] + R[4] + R[8] - 1) * 0.5;
+    c = c > 1. ? 1. : c < -1. ? -1. : c;
+    double theta = acos(c);
+    if (s < 1e-5) {
+        if (c > 0) {
+            rx = ry = rz = 0;
+        } else {
+            rx = sqrt(fmax((R[0] + 1) * 0.5, 0.));
+            ry = sqrt(fmax((R[4] + 1) * 0.5, 0.)) * (R[1] < 0 ? -1. : 1.);
+            rz = sqrt(fmax((R[8] + 1) * 0.5, 0.)) * (R[2] < 0 ? -1. : 1.);
+            if (fabs(rx) < fabs(ry) && fabs(rx) < fabs(rz) && (R[5] > 0) != (ry * rz > 0)) rz = -rz;
+            theta /= sqrt(rx * rx + ry * ry + rz * rz);
+            rx *= theta;
+            ry *= theta;
+            rz *= theta;
+        }
+    } else {
+        const double vth = 1 / (2 * s) * theta;
+        rx *= vth;
+        ry *= vth;
+        rz *= vth;
+    }
+    r[0] = rx;
+    r[1] = ry;
+    r[2] = rz;
+}
+
+// cv::solve(A, b, DECOMP_SVD) for the 6x6 damped normal equations, OpenCV's back-substitution threshold (as svd_lstsq6)
+__device__ void svd_solve6(LmShared& L, const double* b, double* x) {
+    for (int j = 0; j < 6; ++j)
+        for (int i = 0; i < 6; ++i) L.At[j * 6 + i] = L.JtJ[i * 6 + j] * (i == j ? 1.0 + exp(L.lam * log(10.)) : 1.0);
+    jacobi_svd(L.At, 6, L.w, L.Vt, 6, 6, 6);
+    double thr = 0;
+    for (int j = 0; j < 6; ++j) thr += L.w[j];
+    thr *= 2.220446049250313e-16 * 2;
+    for (int k = 0; k < 6; ++k) x[k] = 0;
+    for (int j = 0; j < 6; ++j) {
+        if (fabs(L.w[j]) <= thr) continue;
+        double ub = 0;
+        for (int i = 0; i < 6; ++i) ub += L.At[j * 6 + i] * b[i];
+        ub /= L.w[j];
+        for (int k = 0; k < 6; ++k) x[k] += ub * L.Vt[j * 6 + k];
+    }
+}
+
+// CvLevMarq::step: p = prev - solve(JtJ with its diagonal * (1 + 10^lam), Jtr); then R, dR/dr at the new p (thread 0)
+__device__ void lm_step(LmShared& L) {
+    double x[6];
+    svd_solve6(L, L.Jtr, x);
+    for (int k = 0; k < 6; ++k) L.p[k] = L.prev[k] - x[k];
+    rodrigues_v2m(L.p, L.R, L.dRdr);
+}
+
+// Residual of one point (model point q[0:3], image point q[3:5]) at (L.R, L.p[3:6]); with J: its two Jacobian rows
+template <bool WANT_J>
+__device__ __forceinline__ void lm_point(const LmShared& L, const Cam& cam, const double* q, double& ru, double& rv, double* ju,
+                                         double* jv) {
+    const double X = q[0], Y = q[1], Z = q[2];
+    const double Xc = L.R[0] * X + L.R[1] * Y + L.R[2] * Z + L.p[3];
+    const double Yc = L.R[3] * X + L.R[4] * Y + L.R[5] * Z + L.p[4];
+    const double Zc = L.R[6] * X + L.R[7] * Y + L.R[8] * Z + L.p[5];
+    const double z = Zc != 0.0 ? 1.0 / Zc : 1.0;
+    const double x = Xc * z, y = Yc * z;
+    ru = cam.fu * x + cam.uc - q[3];
+    rv = cam.fv * y + cam.vc - q[4];
+    if (WANT_J) {
+#pragma unroll
+        for (int j = 0; j < 3; ++j) {
+            const double* d = L.dRdr + 9 * j;
+            const double dX = X * d[0] + Y * d[1] + Z * d[2];
+            const double dY = X * d[3] + Y * d[4] + Z * d[5];
+            const double dZ = X * d[6] + Y * d[7] + Z * d[8];
+            ju[j] = cam.fu * (z * (dX - x * dZ));
+            jv[j] = cam.fv * (z * (dY - y * dZ));
+        }
+        ju[3] = cam.fu * z;
+        ju[4] = 0.0;
+        ju[5] = cam.fu * (-x * z);
+        jv[3] = 0.0;
+        jv[4] = cam.fv * z;
+        jv[5] = cam.fv * (-y * z);
+    }
+}
+
+// CALC_J: JtJ (21 unique entries), Jtr, |r|^2 over all points in one reduction; thread 0 then takes the damped step
+template <int NT>
+__device__ void lm_calc_j(const double* P, int n, const Cam& cam, LmShared& L, EpnpShared& S) {
+    double v[28];
+#pragma unroll
+    for (int k = 0; k < 28; ++k) v[k] = 0;
+    for (int i = threadIdx.x; i < n; i += NT) {
+        // re-read R / dRdr from shared memory per point: hoisted next to the 28 accumulators they spill to local memory
+        asm volatile("" ::: "memory");
+        double ru, rv, ju[6], jv[6];
+        lm_point<true>(L, cam, P + (long)i * 5, ru, rv, ju, jv);
+        int e = 0;
+#pragma unroll
+        for (int a = 0; a < 6; ++a) {
+#pragma unroll
+            for (int c = a; c < 6; ++c) v[e++] += ju[a] * ju[c] + jv[a] * jv[c];
+            v[21 + a] += ju[a] * ru + jv[a] * rv;
+        }
+        v[27] += ru * ru + rv * rv;
+    }
+    block_sum<NT, 28>(v, S);
+    if (threadIdx.x == 0) {
+        int e = 0;
+        for (int a = 0; a < 6; ++a) {
+            for (int c = a; c < 6; ++c, ++e) L.JtJ[a * 6 + c] = L.JtJ[c * 6 + a] = S.sums[e];
+            L.Jtr[a] = S.sums[21 + a];
+            L.prev[a] = L.p[a];
+        }
+        if (L.iters == 0) L.prev_err = sqrt(S.sums[27]);
+        lm_step(L);
+    }
+    __syncthreads();
+}
+
+// Per-ROI scratch: the gathered points of pnp_gather_kernel.  R_init [B][3][3], t_init [B][3] = the network pose (float32).
+__global__ void __launch_bounds__(kPnpThreads) pnp_lm_kernel(const double* __restrict__ pts, const int* __restrict__ counts,
+                                                            const float* __restrict__ K, const float* __restrict__ R_init,
+                                                            const float* __restrict__ t_init, int HW, int max_iters,
+                                                            float* __restrict__ out_pose, int* __restrict__ out_info) {
+    const int b = blockIdx.x, tid = threadIdx.x;
+    const int n = counts[b];
+    __shared__ EpnpShared S;
+    __shared__ LmShared L;
+    if (n < 4) {  // cv2 refuses fewer than 4 points without a guess; the evaluator keeps the network pose below 4
+        for (int e = tid; e < 12; e += kPnpThreads) out_pose[b * 12 + e] = (e & 3) < 3 ? R_init[b * 9 + 3 * (e >> 2) + (e & 3)] : t_init[b * 3 + (e >> 2)];
+        if (tid == 0) {
+            out_info[b * 4 + 0] = n;
+            out_info[b * 4 + 1] = 0;
+            out_info[b * 4 + 2] = 0;
+            out_info[b * 4 + 3] = 0;
+        }
+        return;
+    }
+    const double* P = pts + (long)b * HW * 5;
+    const Cam cam = load_cam(K, b);
+    if (tid == 0) {
+        // rvec0 = cv2.Rodrigues(R_net) on the float32 rotation: computed in double, handed back in float32
+        double R0[9], r0[3];
+        for (int k = 0; k < 9; ++k) R0[k] = (double)R_init[b * 9 + k];
+        rodrigues_m2v(R0, r0, L.At, L.Vt, L.w);
+        for (int k = 0; k < 3; ++k) {
+            L.p[k] = (double)(float)r0[k];
+            L.p[3 + k] = (double)t_init[b * 3 + k];
+        }
+        rodrigues_v2m(L.p, L.R, L.dRdr);
+        L.lam = -3;
+        L.iters = 0;
+    }
+    __syncthreads();
+    lm_calc_j<kPnpThreads>(P, n, cam, L, S);
+    for (;;) {
+        double v[1] = {0};
+        for (int i = tid; i < n; i += kPnpThreads) {
+            double ru, rv;
+            lm_point<false>(L, cam, P + (long)i * 5, ru, rv, nullptr, nullptr);
+            v[0] += ru * ru + rv * rv;
+        }
+        block_sum<kPnpThreads, 1>(v, S);
+        if (tid == 0) {
+            const double err = sqrt(S.sums[0]);
+            L.phase = 0;
+            if (!(err > L.prev_err && ++L.lam <= 16)) {
+                L.lam = L.lam - 1 > -16 ? L.lam - 1 : -16;
+                double dn = 0, pn = 0;
+                for (int k = 0; k < 6; ++k) {
+                    dn += (L.p[k] - L.prev[k]) * (L.p[k] - L.prev[k]);
+                    pn += L.prev[k] * L.prev[k];
+                }
+                if (++L.iters >= max_iters || sqrt(dn) / (sqrt(pn) + 2.220446049250313e-16) < 1.1920928955078125e-07) {
+                    L.phase = 2;
+                } else {
+                    L.prev_err = err;
+                    L.phase = 1;
+                }
+            } else {
+                lm_step(L);  // error went up: more damping, same Jacobian
+            }
+        }
+        __syncthreads();
+        const int phase = L.phase;
+        if (phase == 2) break;
+        if (phase == 1) lm_calc_j<kPnpThreads>(P, n, cam, L, S);
+    }
+    if (tid == 0) {
+        // the evaluator passes float32 guess arrays, into which cv2 writes the solution; R = cv2.Rodrigues(rvec)
+        double r[3];
+        for (int k = 0; k < 3; ++k) r[k] = (double)(float)L.p[k];
+        rodrigues_v2m(r, L.R, L.dRdr);
+        for (int e = 0; e < 12; ++e) {
+            const int i = e >> 2, c = e & 3;
+            out_pose[b * 12 + e] = c < 3 ? (float)L.R[3 * i + c] : (float)L.p[3 + i];
+        }
+        out_info[b * 4 + 0] = n;
+        out_info[b * 4 + 1] = L.iters;
+        out_info[b * 4 + 2] = 1;
+        out_info[b * 4 + 3] = 0;
+    }
+}
+
 }  // namespace
 }  // namespace gdrn
+
+extern "C" long gdrn_pnp_iterative_workspace_bytes(int B, int HW) {
+    size_t n = 0;
+    n += (size_t)B * HW * 5 * sizeof(double);  // points
+    n += (size_t)B * sizeof(int);              // counts
+    return (long)(n + 256);
+}
+
+extern "C" int gdrn_pnp_iterative(const float* mask, const float* xyz, const float* coord2d, const float* extents, const float* im_wh,
+                                  const float* K, const float* R_init, const float* t_init, int B, int H, int W, int mask_mode,
+                                  float mask_thr, int max_iters, void* workspace, long workspace_bytes, float* out_pose, int* out_info,
+                                  void* stream_) {
+    using namespace gdrn;
+    cudaStream_t stream = (cudaStream_t)stream_;
+    if (!mask || !xyz || !coord2d || !extents || !im_wh || !K || !R_init || !t_init || !workspace || !out_pose || !out_info)
+        return set_error(GDRN_ERR_ARG, "gdrn_pnp_iterative: null pointer");
+    if (B <= 0 || H <= 0 || W <= 0 || max_iters <= 0 || max_iters > 1000 || mask_mode < 0 || mask_mode > 2)
+        return set_error(GDRN_ERR_ARG, "gdrn_pnp_iterative: bad sizes (B=%d H=%d W=%d max_iters=%d mask_mode=%d)", B, H, W, max_iters,
+                         mask_mode);
+    const int HW = H * W;
+    if (workspace_bytes < gdrn_pnp_iterative_workspace_bytes(B, HW))
+        return set_error(GDRN_ERR_ARG, "gdrn_pnp_iterative: workspace too small (%ld < %ld)", workspace_bytes,
+                         gdrn_pnp_iterative_workspace_bytes(B, HW));
+    if ((reinterpret_cast<uintptr_t>(workspace) & 7) != 0)
+        return set_error(GDRN_ERR_ARG, "gdrn_pnp_iterative: workspace must be 8-byte aligned");
+    double* pts = (double*)workspace;
+    int* counts = (int*)((char*)workspace + (size_t)B * HW * 5 * sizeof(double));
+    GDRN_LAUNCH(pnp_gather_kernel, dim3(B), dim3(kGatherThreads), stream, mask, xyz, coord2d, extents, im_wh, HW, mask_mode, mask_thr, pts,
+                counts);
+    GDRN_CUDA_OK(cudaGetLastError());
+    count_launch();
+    GDRN_LAUNCH(pnp_lm_kernel, dim3(B), dim3(kPnpThreads), stream, pts, counts, K, R_init, t_init, HW, max_iters, out_pose, out_info);
+    GDRN_CUDA_OK(cudaGetLastError());
+    count_launch();
+    return GDRN_OK;
+}
 
 extern "C" long gdrn_pnp_ransac_workspace_bytes(int B, int HW, int iters) {
     size_t n = 0;

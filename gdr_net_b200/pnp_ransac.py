@@ -6,7 +6,12 @@ host: `get_out_coor` / `get_out_mask` (`engine_utils.py:92-126`), D2H copies, `g
 replaces the translation by the one decoded from the network's (cx, cy, z) head (:398-421).
 
 Here the whole batch is solved by three kernel launches (`csrc/pnp_ransac.cu`), following OpenCV's algorithm closely enough that
-the inlier sets and poses agree with cv2 up to round-off (tests/test_pnp_ransac_gpu.py).  No host synchronisation."""
+the inlier sets and poses agree with cv2 up to round-off (tests/test_pnp_ransac_gpu.py).  No host synchronisation.
+
+The network-initialised modes of the evaluator (`process_net_and_pnp`, gdrn_evaluator.py:187-314: TEST.PNP_TYPE net_iter_pnp,
+net_ransac_pnp, net_ransac_pnp_rot) are `process_net_and_pnp` below: the iterative one is OpenCV's Levenberg-Marquardt
+(`pnp_iterative`, two launches), the RANSAC ones reuse `pnp_ransac` with 20 iterations.  `process_pnp` dispatches on the
+config like the evaluator does."""
 from __future__ import annotations
 
 import torch
@@ -69,3 +74,107 @@ def process_pnp_ransac(out_dict: dict, roi_coord_2d: torch.Tensor, roi_extents: 
     if use_net_trans:
         pose[:, :, 3] = out_dict["trans"].to(pose.dtype)
     return pose
+
+
+def _net_pose(out_dict: dict) -> tuple:
+    R = out_dict["rot"].detach().float().reshape(-1, 3, 3).contiguous()
+    t = out_dict["trans"].detach().float().reshape(-1, 3).contiguous()
+    return R, t
+
+
+def pnp_iterative(mask: torch.Tensor, xyz: torch.Tensor, coord_2d: torch.Tensor, extents: torch.Tensor, im_wh, cams: torch.Tensor,
+                  R_init: torch.Tensor, t_init: torch.Tensor, mask_loss_type: str = "L1", mask_thr: float = 0.5,
+                  max_iters: int = 20) -> dict:
+    """cv2.solvePnP(SOLVEPNP_ITERATIVE, useExtrinsicGuess=True) for the whole batch on the device: OpenCV's Levenberg-Marquardt
+    refinement of the reprojection error, started at (R_init [B,3,3], t_init [B,3]).  Points are selected like `pnp_ransac`, whose
+    argument conventions this follows.  Like the evaluator's call, whose guess arrays are float32, the start rotation vector and
+    the solution are rounded to float32 before R is formed.
+    Returns dict(pose [B,3,4], num_points [B], iterations [B] (accepted LM steps), ok [B] (bool)).  Instances with fewer than 4
+    selected points get ok = False and the initial pose."""
+    if not mask.is_cuda:
+        raise RuntimeError("gdr_net_b200.pnp_iterative runs on CUDA only; there is no CPU fallback")
+    if mask_loss_type not in _MASK_MODES:
+        raise NotImplementedError(f"unknown mask loss type: {mask_loss_type}")
+    dev = mask.device
+    B, _, h, w = xyz.shape
+    f = lambda t: t.detach().to(dev).float().contiguous()  # noqa: E731
+    mask, xyz, coord_2d, extents = f(mask).reshape(B, h * w), f(xyz), f(coord_2d), f(extents).reshape(B, 3)
+    if coord_2d.shape != (B, 2, h, w):
+        raise ValueError(f"pnp_iterative: coord_2d {tuple(coord_2d.shape)} does not match xyz {tuple(xyz.shape)}")
+    R_init, t_init = f(R_init).reshape(B, 3, 3), f(t_init).reshape(B, 3)
+    if not torch.is_tensor(im_wh):
+        im_wh = torch.tensor(im_wh, dtype=torch.float32)
+    im_wh = f(im_wh)
+    im_wh = (im_wh.reshape(1, 2).expand(B, 2) if im_wh.numel() == 2 else im_wh.reshape(B, 2)).contiguous()
+    cams = f(cams)
+    cams = (cams.reshape(1, 3, 3).expand(B, 3, 3) if cams.dim() == 2 else cams.reshape(B, 3, 3)).contiguous()
+    nbytes = int(C.load().gdrn_pnp_iterative_workspace_bytes(B, h * w))
+    ws = torch.empty((nbytes + 7) // 8, dtype=torch.float64, device=dev)
+    pose = torch.empty(B, 3, 4, device=dev)
+    info = torch.empty(B, 4, dtype=torch.int32, device=dev)
+    C.gdrn_pnp_iterative(mask.data_ptr(), xyz.data_ptr(), coord_2d.data_ptr(), extents.data_ptr(), im_wh.data_ptr(), cams.data_ptr(),
+                         R_init.data_ptr(), t_init.data_ptr(), B, h, w, _MASK_MODES[mask_loss_type], float(mask_thr), int(max_iters),
+                         ws.data_ptr(), ws.numel() * 8, pose.data_ptr(), info.data_ptr(), torch.cuda.current_stream().cuda_stream)
+    return dict(pose=pose, num_points=info[:, 0], iterations=info[:, 1], ok=info[:, 2] != 0)
+
+
+def process_net_and_pnp(out_dict: dict, roi_coord_2d: torch.Tensor, roi_extents: torch.Tensor, im_wh, cams: torch.Tensor,
+                        pnp_type: str = "iter", mask_loss_type: str = "L1", mask_thr: float = 0.5) -> torch.Tensor:
+    """Batched equivalent of the pose part of `process_net_and_pnp` (gdrn_custom_evaluator.py:207-335, gdrn_evaluator.py:187-314):
+    PnP on the predicted coordinate maps, initialised with the network pose (out_dict["rot"] [B,3,3], out_dict["trans"] [B,3]).
+
+      * "iter":       cv2.solvePnP(ITERATIVE, useExtrinsicGuess) -> `pnp_iterative`; R and t from PnP;
+      * "ransac":     cv2.solvePnPRansac(EPNP, 3 px, 20 iterations) -> `pnp_ransac(iters=20)` (EPnP ignores the guess); R and
+                      t from PnP, but the network's t where |t_pnp - t_net| > 1 m;
+      * "ransac_rot": as "ransac", t always from the network.
+
+    Fewer than 4 selected points, or a failed RANSAC: the network pose.  The reference's `te > 1` fallback is not applied in
+    "iter" mode because it never fires there: cv2 writes the solution into the float32 guess array that the reference then
+    compares it with.  Deviation: with exactly 4 points OpenCV's RANSAC switches to P3P, which has no device kernel here; those
+    instances keep the network pose in the two RANSAC modes ("iter" runs the LM on 4 points like cv2).
+    Returns [B,3,4] float32, computed on the device without host synchronisation (capturable in a CUDA graph)."""
+    R_net, t_net = _net_pose(out_dict)
+    xyz = torch.cat([out_dict["coor_x"], out_dict["coor_y"], out_dict["coor_z"]], dim=1)
+    if pnp_type == "iter":
+        res = pnp_iterative(out_dict["mask"], xyz, roi_coord_2d, roi_extents, im_wh, cams, R_net, t_net, mask_loss_type=mask_loss_type,
+                            mask_thr=mask_thr)
+    elif pnp_type in ("ransac", "ransac_rot"):
+        res = pnp_ransac(out_dict["mask"], xyz, roi_coord_2d, roi_extents, im_wh, cams, mask_loss_type=mask_loss_type,
+                         mask_thr=mask_thr, iters=20)
+    else:
+        raise NotImplementedError(f"unknown net + PnP type: {pnp_type}")
+    return combine_net_and_pnp(pnp_type, R_net, t_net, res["pose"], res["ok"])
+
+
+def combine_net_and_pnp(pnp_type: str, R_net: torch.Tensor, t_net: torch.Tensor, pnp_pose: torch.Tensor, pnp_ok: torch.Tensor):
+    """The per-ROI rules of `process_net_and_pnp` as tensor operations (any device, no host reads): R_net [B,3,3], t_net [B,3],
+    pnp_pose [B,3,4], pnp_ok [B] bool -> [B,3,4]."""
+    ok = pnp_ok.view(-1)
+    R = torch.where(ok.view(-1, 1, 1), pnp_pose[:, :, :3], R_net)
+    t_pnp = pnp_pose[:, :, 3]
+    if pnp_type == "iter":
+        use_t = ok
+    elif pnp_type == "ransac":
+        use_t = ok & ((t_pnp.double() - t_net.double()).norm(dim=1) <= 1.0)
+    else:
+        use_t = torch.zeros_like(ok)
+    t = torch.where(use_t.view(-1, 1), t_pnp, t_net)
+    return torch.cat([R, t.unsqueeze(-1)], dim=-1)
+
+
+_NET_PNP_TYPES = {"net_iter_pnp": "iter", "net_ransac_pnp": "ransac", "net_ransac_pnp_rot": "ransac_rot"}
+
+
+def process_pnp(cfg, out_dict: dict, roi_coord_2d: torch.Tensor, roi_extents: torch.Tensor, im_wh, cams: torch.Tensor) -> torch.Tensor:
+    """The evaluator's `TEST.USE_PNP` dispatch (gdrn_custom_evaluator.py:160-171) on `cfg.TEST.PNP_TYPE` (case-insensitive):
+    "ransac_pnp" -> `process_pnp_ransac`; "net_iter_pnp" / "net_ransac_pnp" / "net_ransac_pnp_rot" -> `process_net_and_pnp`
+    with "iter" / "ransac" / "ransac_rot"; anything else raises NotImplementedError.  The mask head type and threshold come
+    from cfg.MODEL.CDPN.ROT_HEAD (MASK_LOSS_TYPE, MASK_THR_TEST).  Returns the [B,3,4] poses."""
+    pnp_type = cfg.TEST.PNP_TYPE.lower()
+    r = cfg.MODEL.CDPN.ROT_HEAD
+    kw = dict(mask_loss_type=r.MASK_LOSS_TYPE, mask_thr=r.MASK_THR_TEST)
+    if pnp_type == "ransac_pnp":
+        return process_pnp_ransac(out_dict, roi_coord_2d, roi_extents, im_wh, cams, **kw)
+    if pnp_type in _NET_PNP_TYPES:
+        return process_net_and_pnp(out_dict, roi_coord_2d, roi_extents, im_wh, cams, pnp_type=_NET_PNP_TYPES[pnp_type], **kw)
+    raise NotImplementedError(f"unknown TEST.PNP_TYPE: {cfg.TEST.PNP_TYPE}")

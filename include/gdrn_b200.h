@@ -198,6 +198,18 @@ int gdrn_pnp_ransac(const float* mask, const float* xyz, const float* coord2d, c
                     double confidence, void* workspace, long workspace_bytes, float* out_pose, int* out_info,
                     unsigned char* out_inliers, void* stream);
 
+/* ---- network-initialised iterative PnP of the evaluator (TEST.PNP_TYPE net_iter_pnp, gdrn_evaluator.py:187-314
+ * `process_net_and_pnp`: cv2.solvePnP(SOLVEPNP_ITERATIVE, useExtrinsicGuess=True) started at the network pose, per instance on
+ * the host).  Inputs as gdrn_pnp_ransac, plus R_init [B][3][3] / t_init [B][3] = the network pose.  OpenCV's Levenberg-Marquardt
+ * (cvFindExtrinsicCameraParams2 + CvLevMarq, at most max_iters accepted steps, 20 in OpenCV) in fp64, one CTA per instance:
+ * the same minimiser and iteration count as cv2.  The solution is rounded to float32 before R is formed, as the reference's
+ * float32 guess arrays do.  out_pose [B][3][4] = [R | t]; out_info [B][4] = (selected points, iterations, ok, 0); fewer than 4
+ * points: ok = 0 and out_pose = the initial pose. */
+long gdrn_pnp_iterative_workspace_bytes(int B, int HW);
+int gdrn_pnp_iterative(const float* mask, const float* xyz, const float* coord2d, const float* extents, const float* im_wh,
+                       const float* K, const float* R_init, const float* t_init, int B, int H, int W, int mask_mode, float mask_thr,
+                       int max_iters, void* workspace, long workspace_bytes, float* out_pose, int* out_info, void* stream);
+
 /* ---- fused Ranger step (gradient centralisation + RAdam + Lookahead), lib/torch_utils/solver/ranger.py:100-200, for all
  * tensors of a param group in ONE launch.  jobs: device array of 64-byte records {float* p; const float* g; float* m; float* v;
  * float* slow; long numel; int row_len; int pad[3]} (row_len > 0: centralise rows of that length);
