@@ -14,27 +14,15 @@ precision = "mixed"  : the fp32x3 forward (every output / loss inside the 1e-3 p
 """
 from __future__ import annotations
 
-from typing import Dict, List, Optional
+import os
+from typing import Dict, Optional
 
 import torch
 
 from . import ops
 from .capi import C
 from .ops import PT, _stream
-
-import os
-
-_DGRAD_ZERO_INSERT = os.environ.get("GDRN_DGRAD_ZERO_INSERT") == "1"  # A/B switch: the first (zero-insert + s1 conv) s2 dgrad
-
-# A/B switch: recompute the ReLU mask of plain conv-BN-ReLU layers from u instead of reading y back in BN backward.
-# MEASURED (same box, graphed step): 11.39-11.47 ms with the recompute vs 11.11-11.33 ms reading y -- 2 B/element less HBM
-# traffic does not pay for the extra per-element FMA + compare + shared-memory constants, so it is off.
-_BN_MASK_FROM_U = os.environ.get("GDRN_BN_MASK_FROM_U") == "1"
-# A/B switch: ConvTranspose2d forward / wgrad by output-parity phases over the un-dilated input (default) instead of a
-# stride-1 conv over the zero-inserted input (4x the MACs + a zero_insert pass)
-_DECONV_PHASES = os.environ.get("GDRN_DECONV_PHASES", "1") == "1"
-# A/B switch: BatchNorm forward emits the ReLU mask as a bitmap that backward reads instead of the activation (default on)
-_BN_BITMASK = os.environ.get("GDRN_BN_BITMASK", "1") == "1"
+from .patch_pnp import pnp_net_forward
 
 LOSS_NAMES = ["loss_coor_x", "loss_coor_y", "loss_coor_z", "loss_mask", "loss_region", "loss_PM_R", "loss_centroid", "loss_z"]
 HEAD_CONVS = [(3, 4, False), (6, 7, False), (10, 11, True), (13, 14, False), (17, 18, True), (20, 21, False)]
@@ -116,7 +104,7 @@ class Engine:
             raise RuntimeError("gdr_net_b200 engine needs CUDA parameters (model.to('cuda')); no CPU fallback exists")
         self.ws = ops.Workspace(self.dev)
         self.sym_table = SymTable(self.dev)
-        self.wgrad_side_stream = os.environ.get("GDRN_WGRAD_STREAM", "1") == "1"
+        self.wgrad_side_stream = True  # weight gradients and the weight pack on a second stream (_on_side)
         self._side_stream, self._side_keep = None, []
         # BatchNorm batch statistics and backward sums in two ordered stages (default) instead of fp32 atomics in the GEMM
         # epilogue: the same inputs give the same step every run.  With atomics the ~1e-7 jitter of the statistics flips
@@ -124,7 +112,7 @@ class Engine:
         # tensor in forward (3 % of the B = 64 step on an H100).  GDRN_DETERMINISTIC=0 selects the atomics.
         self.deterministic = os.environ.get("GDRN_DETERMINISTIC", "1") == "1"
         self._det_ws = None
-        self.fold_eval = os.environ.get("GDRN_NO_FOLD_EVAL") != "1"  # A/B switch: eval forward through the unfused train-path kernels
+        self.fold_eval = True  # inference by forward_eval_folded; False runs it through the unfused train-path kernels
         self.with_2d = int(model.pnp_net.features[0].in_channels == 69)  # 69 = xyz + coord2d + regions, 67 without coords
         assert model.pnp_net.features[0].in_channels in (67, 69), model.pnp_net.features[0].in_channels
         self.named_params = list(model.named_parameters())
@@ -167,8 +155,9 @@ class Engine:
 
     # ------------------------------------------------------------------------------------------ weights
     def _conv_modules(self):
+        """(key, module) of every conv packed by pack_conv_fwd; the 7x7 stem is a GEMM over its im2col matrix (pack_stem)."""
         m = self.model
-        out = [("backbone.conv1", m.backbone.conv1)]
+        out = []
         for li in range(1, 5):
             for bi, blk in enumerate(getattr(m.backbone, f"layer{li}")):
                 p = f"backbone.layer{li}.{bi}"
@@ -186,8 +175,6 @@ class Engine:
     def prepare_weights(self, need_dgrad: bool):
         """fp32 parameters -> K-major bf16 (hi, lo) GEMM operands, re-done every step (weights change) by ONE batched
         launch over a device-resident job table (rebuilt only if a parameter / buffer pointer moved)."""
-        import numpy as np
-
         key = (need_dgrad, tuple(p.data_ptr() for _, p in self.named_params))
         tables = self.__dict__.setdefault("_pack_tables", {})
         tab = tables.get(key)
@@ -195,29 +182,37 @@ class Engine:
             # One persistent job table per (need_dgrad, parameter addresses).  Tables are NEVER freed or overwritten: a
             # captured CUDA graph holds the raw device pointer of the table it was captured with, and an eager call with
             # the other need_dgrad value (train -> eval -> train) must not invalidate it (ADVICE r1).
-            ops._pack_recorder = []
-            try:
-                self._prepare_weights_calls(need_dgrad)
-                self._pack_stem()
-                jobs = ops._pack_recorder
-            finally:
-                ops._pack_recorder = None
-            dt = np.dtype([("src", "<u8"), ("hi", "<u8"), ("lo", "<u8"), ("so", "<i8"), ("si", "<i8"), ("sr", "<i8"), ("ss", "<i8"),
-                           ("begin", "<i8"), ("O", "<i4"), ("I", "<i4"), ("KH", "<i4"), ("KW", "<i4"), ("opad", "<i4"),
-                           ("ipad", "<i4"), ("krow", "<i4"), ("flip", "<i4"), ("row_scale", "<u8")])
-            assert dt.itemsize == 104
-            arr = np.zeros(len(jobs), dtype=dt)
-            begin = 0
-            for n, (src, out, O, I, KH, KW, opad, ipad, krow, so, si, sr, ss, flip) in enumerate(jobs):
-                arr[n] = (src.data_ptr(), out.hi_ptr, out.lo_ptr or 0, so, si, sr, ss, begin, O, I, KH, KW, opad, ipad, krow, flip, 0)
-                begin += -(-opad // 16) * -(-ipad // 64) * -(-(KH * KW) // 9)  # tiles of 16 rows x 64 channels x 9 taps (pack.cu)
-            tab = dict(jobs=torch.from_numpy(arr.view(np.uint8).copy()).to(self.dev), njobs=len(jobs), blocks=begin,
-                       keep=[j[0] for j in jobs] + [j[1] for j in jobs])  # sources and destinations stay alive with the table
-            tables[key] = tab
+            tab = tables[key] = self._pack_table(lambda: self._prepare_weights_calls(need_dgrad))
         with torch.no_grad():
             torch.cat([self.model.pnp_net.fc_r.weight, self.model.pnp_net.fc_t.weight], 0, out=self.w_rt)
             torch.cat([self.model.pnp_net.fc_r.bias, self.model.pnp_net.fc_t.bias], 0, out=self.b_rt)
         C.gdrn_pack_weight_batched(tab["jobs"].data_ptr(), tab["njobs"], tab["blocks"], _stream())
+
+    def _pack_table(self, pack, row_scales=None) -> dict:
+        """Runs pack() with its ops.pack_* calls recorded instead of launched and returns them as the device job table of
+        gdrn_pack_weight_batched (jobs, njobs, blocks).  row_scales[n], if given, multiplies every output row of job n.
+        The table keeps the jobs' sources and destinations alive."""
+        import numpy as np
+
+        ops._pack_recorder = []
+        try:
+            pack()
+            jobs = ops._pack_recorder
+        finally:
+            ops._pack_recorder = None
+        assert row_scales is None or len(row_scales) == len(jobs)
+        dt = np.dtype([("src", "<u8"), ("hi", "<u8"), ("lo", "<u8"), ("so", "<i8"), ("si", "<i8"), ("sr", "<i8"), ("ss", "<i8"),
+                       ("begin", "<i8"), ("O", "<i4"), ("I", "<i4"), ("KH", "<i4"), ("KW", "<i4"), ("opad", "<i4"),
+                       ("ipad", "<i4"), ("krow", "<i4"), ("flip", "<i4"), ("row_scale", "<u8")])  # struct PackJob (pack.cu)
+        assert dt.itemsize == 104
+        arr = np.zeros(len(jobs), dtype=dt)
+        begin = 0
+        for n, (src, out, O, I, KH, KW, opad, ipad, krow, so, si, sr, ss, flip) in enumerate(jobs):
+            scale = 0 if row_scales is None else row_scales[n].data_ptr()
+            arr[n] = (src.data_ptr(), out.hi_ptr, out.lo_ptr or 0, so, si, sr, ss, begin, O, I, KH, KW, opad, ipad, krow, flip, scale)
+            begin += -(-opad // 16) * -(-ipad // 64) * -(-(KH * KW) // 9)  # tiles of 16 rows x 64 channels x 9 taps (pack.cu)
+        return dict(jobs=torch.from_numpy(arr.view(np.uint8).copy()).to(self.dev), njobs=len(jobs), blocks=begin,
+                    keep=[j[0] for j in jobs] + [j[1] for j in jobs])
 
     # ------------------------------------------------------------------------------------------ eval: folded conv+BN+ReLU
     # (conv key, BatchNorm key) of every conv that is followed by a BatchNorm, in forward order
@@ -243,7 +238,7 @@ class Engine:
         key = tuple(p.data_ptr() for _, p in self.named_params)
         fold = getattr(self, "_fold", None)
         if fold is None or fold["key"] != key:
-            pl = self.planes
+            m, pl = self.model, self.planes
             pairs = self._conv_bn_pairs()
             convs = dict(self._conv_modules())
             wfe, sc, sh = {}, {}, {}
@@ -257,36 +252,19 @@ class Engine:
                 sh[bk] = torch.empty(mod.num_features, device=self.dev)
                 farr[n] = (mod.weight.data_ptr(), mod.bias.data_ptr(), mod.running_mean.data_ptr(), mod.running_var.data_ptr(),
                            sc[bk].data_ptr(), sh[bk].data_ptr(), mod.num_features, float(mod.eps), 0)
-            ops._pack_recorder = []
-            try:
-                scales = []
-                for ck, bk in pairs:
+
+            def pack():  # one job per (conv, BatchNorm) pair, its rows scaled by that BatchNorm's scale
+                for ck, _bk in pairs:
                     if ck == "stem":
-                        w = self.model.backbone.conv1.weight
-                        wfe[ck] = PT((64, 192), pl, device=self.dev, zero=True)
-                        ops._pack(w, wfe[ck], 64, 3, 7, 7, 64, 3, 192, 147, 49, 7, 1, 0)
+                        wfe[ck] = ops.pack_stem(m.backbone.conv1.weight, pl)
                     elif ck == "deconv":
-                        pk = ops.pack_deconv_fwd_phases if _DECONV_PHASES else ops.pack_deconv_fwd
-                        wfe[ck] = pk(self.model.rot_head_net.features[0].weight, pl)
+                        wfe[ck] = ops.pack_conv_dgrad(m.rot_head_net.features[0].weight, pl)  # see _prepare_weights_calls
                     else:
                         wfe[ck] = ops.pack_conv_fwd(convs[ck].weight, pl)
-                    scales.append(sc[bk])
-                jobs = ops._pack_recorder
-            finally:
-                ops._pack_recorder = None
-            dt = np.dtype([("src", "<u8"), ("hi", "<u8"), ("lo", "<u8"), ("so", "<i8"), ("si", "<i8"), ("sr", "<i8"), ("ss", "<i8"),
-                           ("begin", "<i8"), ("O", "<i4"), ("I", "<i4"), ("KH", "<i4"), ("KW", "<i4"), ("opad", "<i4"),
-                           ("ipad", "<i4"), ("krow", "<i4"), ("flip", "<i4"), ("row_scale", "<u8")])
-            assert dt.itemsize == 104
-            arr = np.zeros(len(jobs), dtype=dt)
-            begin = 0
-            for n, (src, out, O, I, KH, KW, opad, ipad, krow, so, si, sr, ss, flip) in enumerate(jobs):
-                arr[n] = (src.data_ptr(), out.hi_ptr, out.lo_ptr or 0, so, si, sr, ss, begin, O, I, KH, KW, opad, ipad, krow, flip,
-                          scales[n].data_ptr())
-                begin += -(-opad // 16) * -(-ipad // 64) * -(-(KH * KW) // 9)
-            fold = self._fold = dict(key=key, wf=wfe, scale=sc, shift=sh, njobs=len(jobs), blocks=begin, nfold=len(pairs),
+
+            fold = self._fold = dict(key=key, wf=wfe, scale=sc, shift=sh, nfold=len(pairs),
                                      fjobs=torch.from_numpy(farr.view(np.uint8).copy()).to(self.dev),
-                                     jobs=torch.from_numpy(arr.view(np.uint8).copy()).to(self.dev), keep=[j[0] for j in jobs])
+                                     **self._pack_table(pack, row_scales=[sc[bk] for _ck, bk in pairs]))
         C.gdrn_bn_fold_batched(fold["fjobs"].data_ptr(), fold["nfold"], _stream())
         C.gdrn_pack_weight_batched(fold["jobs"].data_ptr(), fold["njobs"], fold["blocks"], _stream())
         return fold
@@ -305,12 +283,9 @@ class Engine:
 
         self._on_side(packs)
 
-        def cbr(xin, ck, bk, conv, relu=True, res=None, kind="conv"):
-            if kind == "deconv":
-                if _DECONV_PHASES:
-                    return ops.conv_dgrad_s2(xin, wfe[ck], conv.out_channels, 3, 1, bias=shift[bk], act=2 if relu else 0)
-                return ops.conv_fwd(ops.zero_insert(xin), wfe[ck], conv.out_channels, 3, 3, 1, 1, bias=shift[bk], act=2 if relu else 0,
-                                    res=res, algo_scale=0.25)
+        def cbr(xin, ck, bk, conv, relu=True, res=None):
+            if ck == "deconv":
+                return ops.conv_dgrad_s2(xin, wfe[ck], conv.out_channels, 3, 1, bias=shift[bk], act=2 if relu else 0)
             k, stride, pad = conv.kernel_size[0], conv.stride[0], conv.padding[0]
             return ops.conv_fwd(xin, wfe[ck], conv.out_channels, k, k, stride, pad, bias=shift[bk], act=2 if relu else 0, res=res)
 
@@ -329,7 +304,7 @@ class Engine:
                     idn = cbr(cur, p + ".downsample.0", p + ".downsample.1", blk.downsample[0], relu=False)
                 cur = cbr(a1, p + ".conv2", p + ".bn2", blk.conv2, res=idn)
         hf = m.rot_head_net.features
-        cur = cbr(cur, "deconv", "rot_head_net.features.1", hf[0], kind="deconv")
+        cur = cbr(cur, "deconv", "rot_head_net.features.1", hf[0])
         for ci, bi, up in HEAD_CONVS:
             if up:
                 cur = ops.upsample2x_fwd(cur)
@@ -343,49 +318,38 @@ class Engine:
         key = (tuple(x.shape), want_maps, tuple(sorted((k, tuple(v.shape)) for k, v in tens.items())),
                tuple(p.data_ptr() for _, p in self.named_params))
         cache = self.__dict__.setdefault("_eval_graphs", {})
-        g = cache.get(key)
-        if g is None:
-            st = dict(x=x.clone(), aux={k: (v.clone() if isinstance(v, torch.Tensor) else v) for k, v in aux.items()})
-            side = torch.cuda.Stream()
-            side.wait_stream(torch.cuda.current_stream())
-            with torch.cuda.stream(side):
-                self.forward_eval_folded(st["x"], st["aux"], want_maps=want_maps)
-            torch.cuda.current_stream().wait_stream(side)
-            torch.cuda.synchronize()
-            st["graph"] = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(st["graph"], capture_error_mode=_capture_mode()):
-                st["res"] = self.forward_eval_folded(st["x"], st["aux"], want_maps=want_maps)
+        if key not in cache:
+            inputs = _clone_inputs(x, aux)
+            [(graph, res)] = _capture(self, [lambda: self.forward_eval_folded(*inputs, want_maps=want_maps)], warmup=1)
             if len(cache) > 8:
                 cache.clear()
-            g = cache[key] = st
-        g["x"].copy_(x, non_blocking=True)
-        for k, v in tens.items():
-            g["aux"][k].copy_(v, non_blocking=True)
-        g["graph"].replay()
-        return {k: (v.clone() if isinstance(v, torch.Tensor) else v) for k, v in g["res"].items()}
+            cache[key] = (inputs, graph, res)
+        inputs, graph, res = cache[key]
+        _copy_inputs(*inputs, x, aux)
+        graph.replay()
+        return {k: (v.clone() if isinstance(v, torch.Tensor) else v) for k, v in res.items()}
+
+    def _head_pnp(self, head_in: PT, aux: dict, pnp_saved: Optional[list] = None):
+        """1x1 output conv -> glue -> Patch-PnP (GDRN.py:156-181, conv_pnp_net.py:111-157).  Returns the fp32 logits
+        [B*4096, 72], the Patch-PnP input planes, pred [B, 16] (cols 0..5 rot6d, 6..8 centroid dx, dy and z) and the inputs
+        of the three FC layers; pnp_saved receives the Patch-PnP conv activations (pnp_net_forward)."""
+        m, B, dev = self.model, head_in.shape[0], self.dev
+        logits = torch.empty(B * 4096, 72, device=dev)
+        ops.conv_fwd(head_in, self.wf["rot_head_net.features.23"], 69, 1, 1, 1, 0, out_f32=logits,
+                     bias=m.rot_head_net.features[23].bias, ldc=72, want_planes=False)
+        pnp_in = PT((B, 64, 64, 128), self.planes, device=dev)
+        C.gdrn_head_glue_fwd(logits.data_ptr(), ops.ptr(aux.get("roi_coord_2d")), aux["roi_extents"].data_ptr(), pnp_in.hi_ptr,
+                             pnp_in.lo_ptr, B, 4096, self.with_2d, _stream())
+        pred = torch.zeros(B, 16, device=dev)
+        fc_in = pnp_net_forward(pnp_in, m.pnp_net, self.wf, self.b_rt, pred, pnp_saved)
+        return logits, pnp_in, pred, fc_in
 
     def _tail_inference(self, head_in: PT, aux: dict, want_maps: bool) -> dict:
         """1x1 output conv -> glue -> Patch-PnP -> test-time pose decode (shared by the folded and the plain eval forward)."""
-        m, pl, dev = self.model, self.planes, self.dev
         B = head_in.shape[0]
-        hf, pn, pf = m.rot_head_net.features, m.pnp_net, m.pnp_net.features
-        logits = torch.empty(B * 4096, 72, device=dev)
-        ops.conv_fwd(head_in, self.wf["rot_head_net.features.23"], 69, 1, 1, 1, 0, out_f32=logits, bias=hf[23].bias, ldc=72,
-                     want_planes=False)
-        pnp_in = PT((B, 64, 64, 128), pl, device=dev)
-        C.gdrn_head_glue_fwd(logits.data_ptr(), ops.ptr(aux.get("roi_coord_2d")), aux["roi_extents"].data_ptr(), pnp_in.hi_ptr,
-                             pnp_in.lo_ptr, B, 4096, self.with_2d, _stream())
-        cur = pnp_in
-        for ci, gi in ((0, 1), (3, 4), (6, 7)):
-            u = ops.conv_fwd(cur, self.wf[f"pnp_net.features.{ci}"], 128, 3, 3, 2, 1)
-            gstats = torch.empty(B, 32, 2, device=dev)
-            cur = ops.gn_relu_fwd(u, pf[gi].weight, pf[gi].bias, gstats, G=pf[gi].num_groups, eps=pf[gi].eps)
-        h1 = ops.gemm_fwd(cur.view(B, 8192), self.wf["fc1"], 1024, bias=pn.fc1.bias, act=1)
-        h2 = ops.gemm_fwd(h1, self.wf["fc2"], 256, bias=pn.fc2.bias, act=1)
-        pred = torch.zeros(B, 16, device=dev)
-        ops.gemm_fwd(h2, self.wf["fc_rt"], 9, out_f32=pred, bias=self.b_rt, ldc=16, want_planes=False)
-        out_rot = torch.empty(B, 3, 3, device=dev)
-        out_trans = torch.empty(B, 3, device=dev)
+        logits, _, pred, _ = self._head_pnp(head_in, aux)
+        out_rot = torch.empty(B, 3, 3, device=self.dev)
+        out_trans = torch.empty(B, 3, device=self.dev)
         C.gdrn_pose_loss(pred.data_ptr(), 16, aux["roi_cams"].data_ptr(), aux["roi_centers"].data_ptr(),
                          aux["roi_whs"].data_ptr(), aux["resize_ratios"].data_ptr(), aux["roi_extents"].data_ptr(), None,
                          None, None, None, None, None, None, out_rot.data_ptr(), out_trans.data_ptr(), None, None, None,
@@ -400,13 +364,13 @@ class Engine:
         m, pl, bpl = self.model, self.planes, self.bplanes
         wf, wd = self.wf, self.wd
         for key, conv in self._conv_modules():
-            if key == "backbone.conv1":
-                continue  # the 7x7 stem is a GEMM over its im2col matrix (_pack_stem)
             wf[key] = ops.pack_conv_fwd(conv.weight, pl, out=wf.get(key))
             if need_dgrad:
                 wd[key] = ops.pack_conv_dgrad(conv.weight, bpl, out=wd.get(key))
         dc = m.rot_head_net.features[0]
-        wf["deconv"] = (ops.pack_deconv_fwd_phases if _DECONV_PHASES else ops.pack_deconv_fwd)(dc.weight, pl, out=wf.get("deconv"))
+        # the ConvTranspose2d forward IS the data gradient of the stride-2 conv whose OIHW weight its IOHW weight is:
+        # gdrn_conv_dgrad_s2 evaluates it by output parity over the un-dilated input (no zero-inserted tensor, 1/4 of the MACs)
+        wf["deconv"] = ops.pack_conv_dgrad(dc.weight, pl, out=wf.get("deconv"))
         if need_dgrad:
             wd["deconv"] = ops.pack_deconv_dgrad(dc.weight, bpl, out=wd.get("deconv"))
         pn = m.pnp_net
@@ -420,13 +384,7 @@ class Engine:
             wd["fc1"] = ops.pack_linear(pn.fc1.weight, bpl, out=wd.get("fc1"), nhwc_from=(128, 8, 8), transpose=True)
             wd["fc2"] = ops.pack_linear(pn.fc2.weight, bpl, out=wd.get("fc2"), transpose=True)
             wd["fc_rt"] = ops.pack_linear(self.w_rt, bpl, out=wd.get("fc_rt"), transpose=True)
-
-    def _pack_stem(self):
-        """7x7 stem weight [64][3][7][7] -> [64][192] with k = (r*7+s)*3 + c (matches gdrn_stem_im2col)."""
-        w = self.model.backbone.conv1.weight
-        out = self.wf.get("stem") or PT((64, 192), self.planes, device=self.dev, zero=True)  # cols 147..191 stay zero
-        ops._pack(w, out, 64, 3, 7, 7, 64, 3, 192, 147, 49, 7, 1, 0)
-        self.wf["stem"] = out
+        wf["stem"] = ops.pack_stem(m.backbone.conv1.weight, pl, out=wf.get("stem"))
 
     # ------------------------------------------------------------------------------------------ building blocks
     def _bn_fwd(self, key: str, u: PT, relu: bool, train_bn: bool, res: Optional[PT] = None) -> PT:
@@ -443,7 +401,7 @@ class Engine:
             C.gdrn_bn_stats(u.hi_ptr, u.lo_ptr, self._det_workspace().data_ptr(), st.stats.data_ptr(), count, Cc, _stream())
         y = ops.like(u)
         mask = None
-        if relu and getattr(self, "_want_masks", False) and _BN_BITMASK:
+        if relu and self._want_masks:
             mask = torch.empty(u.numel() // 8, dtype=torch.uint8, device=self.dev)
         self._last_mask = mask
         C.gdrn_bn_fwd(u.hi_ptr, u.lo_ptr, res.hi_ptr if res else None, res.lo_ptr if res else None, y.hi_ptr, y.lo_ptr,
@@ -457,19 +415,14 @@ class Engine:
             self._det_ws = torch.empty(2 * 512 * int(C.load().gdrn_det_parts()), device=self.dev)
         return self._det_ws
 
-    def _conv_bn(self, x: PT, ckey: str, conv, bkey: str, relu: bool, train_bn: bool, res: Optional[PT] = None,
-                 wkey: Optional[str] = None, kind: str = "conv"):
-        st = self.bn[bkey]
-        stats = st.stats if (train_bn and not self.deterministic) else None  # deterministic: statistics from gdrn_bn_stats
+    def _conv_bn(self, x: PT, ckey: str, conv, bkey: str, relu: bool, train_bn: bool, res: Optional[PT] = None):
+        stats = self.bn[bkey].stats if (train_bn and not self.deterministic) else None  # deterministic: from gdrn_bn_stats
         k, stride, pad = conv.kernel_size[0], conv.stride[0], conv.padding[0]
-        if kind == "deconv" and _DECONV_PHASES:
+        if ckey == "deconv":
             u = ops.conv_dgrad_s2(x, self.wf["deconv"], conv.out_channels, 3, 1, stats=stats)
-        elif kind == "deconv":
-            u = ops.conv_fwd(x, self.wf["deconv"], conv.out_channels, 3, 3, 1, 1, stats=stats, algo_scale=0.25)
         else:
-            u = ops.conv_fwd(x, self.wf[wkey or ckey], conv.out_channels, k, k, stride, pad, stats=stats)
-        y = self._bn_fwd(bkey, u, relu, train_bn, res)
-        return u, y
+            u = ops.conv_fwd(x, self.wf[ckey], conv.out_channels, k, k, stride, pad, stats=stats)
+        return u, self._bn_fwd(bkey, u, relu, train_bn, res)
 
     # ------------------------------------------------------------------------------------------ forward
     def run(self, x, *, roi_coord_2d, roi_cams, roi_centers, roi_whs, roi_extents, resize_ratios, gt_xyz=None,
@@ -561,10 +514,9 @@ class Engine:
 
         # ---- a2: geometry head (cdpn_rot_head_region.py:80-135)
         hf = m.rot_head_net.features
-        z = feat if _DECONV_PHASES else ops.zero_insert(feat)
-        u, y = self._conv_bn(z, "deconv", hf[0], "rot_head_net.features.1", True, train_bn, kind="deconv")
+        u, y = self._conv_bn(feat, "deconv", hf[0], "rot_head_net.features.1", True, train_bn)
         if S is not None:
-            S["deconv"] = dict(z=z, u=u, y=y, m=self._last_mask)
+            S["deconv"] = dict(z=feat, u=u, y=y, m=self._last_mask)
             S["head"] = []
         cur = y
         for ci, bi, up in HEAD_CONVS:
@@ -577,45 +529,14 @@ class Engine:
         head_in = cur  # [B,64,64,256]
         if self._nbt:
             torch._foreach_add_(self._nbt, 1)  # all BatchNorm num_batches_tracked counters in one launch
-        logits = torch.empty(B * 4096, 72, device=dev)
-        ops.conv_fwd(head_in, self.wf["rot_head_net.features.23"], 69, 1, 1, 1, 0, out_f32=logits, bias=hf[23].bias, ldc=72,
-                     want_planes=False)
-
-        # ---- a3 + a4: glue and Patch-PnP (GDRN.py:156-181, conv_pnp_net.py:111-157)
-        pnp_in = PT((B, 64, 64, 128), pl, device=dev)
-        C.gdrn_head_glue_fwd(logits.data_ptr(), ops.ptr(aux.get("roi_coord_2d")), aux["roi_extents"].data_ptr(), pnp_in.hi_ptr,
-                             pnp_in.lo_ptr, B, 4096, self.with_2d, _stream())
-        pf = m.pnp_net.features
-        cur = pnp_in
-        pnp_saved = []
-        for ci, gi in ((0, 1), (3, 4), (6, 7)):
-            u = ops.conv_fwd(cur, self.wf[f"pnp_net.features.{ci}"], 128, 3, 3, 2, 1)
-            gstats = torch.empty(B, 32, 2, device=dev)
-            y = ops.gn_relu_fwd(u, pf[gi].weight, pf[gi].bias, gstats, G=pf[gi].num_groups, eps=pf[gi].eps)
-            pnp_saved.append(dict(ci=ci, gi=gi, x_in=cur, u=u, y=y, gstats=gstats))
-            cur = y
-        flat = cur.view(B, 8192)
-        pn = m.pnp_net
-        h1 = ops.gemm_fwd(flat, self.wf["fc1"], 1024, bias=pn.fc1.bias, act=1)
-        h2 = ops.gemm_fwd(h1, self.wf["fc2"], 256, bias=pn.fc2.bias, act=1)
-        pred = torch.zeros(B, 16, device=dev)  # cols 0..5 rot6d, 6..8 (centroid dx, dy, z)
-        ops.gemm_fwd(h2, self.wf["fc_rt"], 9, out_f32=pred, bias=self.b_rt, ldc=16, want_planes=False)
-
-        # ---- a5/a6 pose decode (+ a7..a10 losses)
-        out_rot = torch.empty(B, 3, 3, device=dev)
-        out_trans = torch.empty(B, 3, device=dev)
-        res = dict(rot=out_rot, trans=out_trans, pred=pred)
         if not do_loss:
-            C.gdrn_pose_loss(pred.data_ptr(), 16, aux["roi_cams"].data_ptr(), aux["roi_centers"].data_ptr(),
-                             aux["roi_whs"].data_ptr(), aux["resize_ratios"].data_ptr(), aux["roi_extents"].data_ptr(), None,
-                             None, None, None, None, None, None, out_rot.data_ptr(), out_trans.data_ptr(), None, None, None,
-                             None, B, 0, 0, 0.0, _stream())
-            if want_maps:
-                maps = logits.view(B, 64, 64, 72).permute(0, 3, 1, 2)
-                res.update(mask=maps[:, 0:1], coor_x=maps[:, 1:2], coor_y=maps[:, 2:3], coor_z=maps[:, 3:4], region=maps[:, 4:69])
-            res["logits"] = logits
-            return res
+            return self._tail_inference(head_in, aux, want_maps)
 
+        # ---- a3 + a4: glue and Patch-PnP
+        pnp_saved = []
+        logits, pnp_in, pred, (flat, h1, h2) = self._head_pnp(head_in, aux, pnp_saved)
+
+        # ---- a5/a6 pose decode + a7..a10 losses
         pix_sums = torch.empty(6, dtype=torch.float64, device=dev)
         C.gdrn_pixel_loss_fwd(logits.data_ptr(), aux["gt_xyz"].data_ptr(), aux["gt_mask_visib"].data_ptr(),
                               aux["gt_mask_trunc"].data_ptr(), aux["gt_region"].data_ptr(), pix_sums.data_ptr(), B, 4096, _stream())
@@ -630,9 +551,8 @@ class Engine:
         n_pts = aux["gt_points"].shape[1]
         C.gdrn_loss_finalize(pix_sums.data_ptr(), S["pose_sums"].data_ptr(), S["vis_ps"].data_ptr(), losses.data_ptr(),
                              vis2.data_ptr(), B, 4096, n_pts, _stream())
-        vis = torch.cat([vis2, out_trans_first(S["out_trans"]), pred[0, 6:9], aux["gt_trans"][0], aux["gt_trans_ratio"][0]])
-        res.update(rot=S["out_rot"], trans=S["out_trans"], losses=losses, vis=vis, logits=logits)
-        return res
+        vis = torch.cat([vis2, S["out_trans"][0], pred[0, 6:9], aux["gt_trans"][0], aux["gt_trans_ratio"][0]])
+        return dict(rot=S["out_rot"], trans=S["out_trans"], pred=pred, losses=losses, vis=vis, logits=logits)
 
     def _pose(self, S, gw):
         aux, B, dev = S["aux"], S["B"], self.dev
@@ -662,7 +582,7 @@ class Engine:
     # nothing but the flat gradient buffer.  Issued on a second stream it runs concurrently with dgrad(L) and -- the point --
     # with the HBM-bound BN-bwd(L-1): tensor-bound and bandwidth-bound work overlap instead of serialising.  The streams join
     # at every gradient-bucket boundary (before the loss-scale removal / all-reduce of that bucket) and at the end of backward;
-    # inside a CUDA graph the fork / join become graph edges.  GDRN_WGRAD_STREAM=0 keeps everything on one stream (A/B).
+    # inside a CUDA graph the fork / join become graph edges.  wgrad_side_stream = False keeps everything on one stream.
     def _on_side(self, fn, keep=()):
         if not self.wgrad_side_stream:
             return fn()
@@ -690,20 +610,17 @@ class Engine:
 
     def _dgrad_conv(self, du: PT, conv, wkey: str) -> PT:
         k, stride, pad = conv.kernel_size[0], conv.stride[0], conv.padding[0]
-        if stride == 2 and not _DGRAD_ZERO_INSERT:
+        if stride == 2:
             # four output-parity phases over the un-dilated dY (no zero-inserted tensor, 1/4 of its MACs)
             return ops.conv_dgrad_s2(du, self.wd[wkey], conv.in_channels, k, pad)
-        z = ops.zero_insert(du) if stride == 2 else du
-        return ops.conv_fwd(z, self.wd[wkey], conv.in_channels, k, k, 1, k - 1 - pad, algo_scale=0.25 if stride == 2 else 1.0)
+        return ops.conv_fwd(du, self.wd[wkey], conv.in_channels, k, k, 1, k - 1 - pad)
 
-    def _bn_bwd(self, bkey: str, ga: PT, gb: Optional[PT], y: Optional[PT], u: PT, want_gout=False, relu_from_u=False, mask=None):
-        """mask: the forward's ReLU bitmap (preferred); else the mask comes from the activation y, or (relu_from_u, A/B
-        switch) is recomputed from u for conv-BN-ReLU without a residual."""
+    def _bn_bwd(self, bkey: str, ga: PT, gb: Optional[PT], u: PT, want_gout=False, mask=None):
+        """mask: the forward's ReLU bitmap (_bn_fwd), None for a BatchNorm without ReLU."""
         mod, st = self._bn_mods[bkey], self.bn[bkey]
-        relu_from_u = relu_from_u and _BN_MASK_FROM_U and mask is None
-        return ops.bn_bwd(ga, gb, None if (relu_from_u or mask is not None) else y, u, st.mean, st.invstd, mod.weight, st.sums,
+        return ops.bn_bwd(ga, gb, None, u, st.mean, st.invstd, mod.weight, st.sums,
                           self.grads[bkey + ".weight"], self.grads[bkey + ".bias"], self.saved["train_bn"], want_gout=want_gout,
-                          beta=mod.bias, relu_from_u=relu_from_u, sums_zeroed=True, relu_mask=mask,
+                          beta=mod.bias, sums_zeroed=True, relu_mask=mask,
                           det_ws=self._det_workspace() if self.deterministic else None)
 
     def backward(self, grad_losses: torch.Tensor):
@@ -776,23 +693,18 @@ class Engine:
         # ---- head convs (cdpn_rot_head_region.py:95-125)
         for L in reversed(S["head"]):
             ci, bi = L["ci"], L["bi"]
-            du, _ = self._bn_bwd(f"rot_head_net.features.{bi}", g, None, h(L["y"]), h(L["u"]), relu_from_u=True, mask=L["m"])
+            du, _ = self._bn_bwd(f"rot_head_net.features.{bi}", g, None, h(L["u"]), mask=L["m"])
             self._wgrad_conv(du, h(L["x_in"]), hf[ci], f"rot_head_net.features.{ci}.weight")
             g = self._dgrad_conv(du, hf[ci], f"rot_head_net.features.{ci}")
             if L["up"]:
                 g = ops.upsample2x_bwd(g)
         D = S["deconv"]
-        du, _ = self._bn_bwd("rot_head_net.features.1", g, None, h(D["y"]), h(D["u"]), relu_from_u=True, mask=D["m"])
+        du, _ = self._bn_bwd("rot_head_net.features.1", g, None, h(D["u"]), mask=D["m"])
         def deconv_wgrad(du=du):
-            if _DECONV_PHASES:
-                # d wt[ci][co][r][s] = sum_q x[ci][q] * du[co][2q + (r, s) - 1]: the weight gradient of the stride-2 conv du -> x
-                # with x in the role of dY; its [O = 512][I = 256][3][3] layout IS the ConvTranspose2d IOHW layout (no flip)
-                buf, ks, kss = ops.conv_wgrad(h(D["z"]), du, self.ws, 512, 3, 3, 2, 1)
-                ops.unpack_wgrad(buf, self.grads["rot_head_net.features.0.weight"], 512, 256, 3, 3, 256, ks, kss, 256 * 9, 9, 3, 1)
-                return
-            buf, ks, kss = ops.conv_wgrad(du, h(D["z"]), self.ws, 256, 3, 3, 1, 1)
-            # ConvTranspose2d weight is IOHW [512][256][3][3] with flipped taps relative to the equivalent conv
-            ops.unpack_wgrad(buf, self.grads["rot_head_net.features.0.weight"], 256, 512, 3, 3, 512, ks, kss, 9, 256 * 9, 3, 1, flip=1)
+            # d wt[ci][co][r][s] = sum_q x[ci][q] * du[co][2q + (r, s) - 1]: the weight gradient of the stride-2 conv du -> x
+            # with x in the role of dY; its [O = 512][I = 256][3][3] layout IS the ConvTranspose2d IOHW layout (no flip)
+            buf, ks, kss = ops.conv_wgrad(h(D["z"]), du, self.ws, 512, 3, 3, 2, 1)
+            ops.unpack_wgrad(buf, self.grads["rot_head_net.features.0.weight"], 512, 256, 3, 3, 256, ks, kss, 256 * 9, 9, 3, 1)
 
         self._on_side(deconv_wgrad, keep=(du,))
         g = ops.conv_fwd(du, self.wd["deconv"], 512, 3, 3, 2, 1)  # [B,8,8,512]
@@ -802,14 +714,14 @@ class Engine:
         ga, gb = g, None
         for Lb in reversed(S["blocks"]):
             p, blk = Lb["p"], Lb["blk"]
-            du2, gout = self._bn_bwd(p + ".bn2", ga, gb, h(Lb["out"]), h(Lb["u2"]), want_gout=True, mask=Lb["m2"])
+            du2, gout = self._bn_bwd(p + ".bn2", ga, gb, h(Lb["u2"]), want_gout=True, mask=Lb["m2"])
             self._wgrad_conv(du2, h(Lb["a1"]), blk.conv2, p + ".conv2.weight")
             da1 = self._dgrad_conv(du2, blk.conv2, p + ".conv2")
-            du1, _ = self._bn_bwd(p + ".bn1", da1, None, h(Lb["a1"]), h(Lb["u1"]), relu_from_u=True, mask=Lb["m1"])
+            du1, _ = self._bn_bwd(p + ".bn1", da1, None, h(Lb["u1"]), mask=Lb["m1"])
             self._wgrad_conv(du1, h(Lb["x_in"]), blk.conv1, p + ".conv1.weight")
             dx_main = self._dgrad_conv(du1, blk.conv1, p + ".conv1")
             if blk.downsample is not None:
-                dud, _ = self._bn_bwd(p + ".downsample.1", gout, None, None, h(Lb["ud"]))
+                dud, _ = self._bn_bwd(p + ".downsample.1", gout, None, h(Lb["ud"]))
                 self._wgrad_conv(dud, h(Lb["x_in"]), blk.downsample[0], p + ".downsample.0.weight")
                 dx_ds = self._dgrad_conv(dud, blk.downsample[0], p + ".downsample.0")
                 ga, gb = dx_main, dx_ds
@@ -820,7 +732,7 @@ class Engine:
         g_pool = ops.add2(ga, gb)
         St = S["stem"]
         g_a0 = ops.maxpool_bwd(St["pool_arg"], g_pool)
-        du0, _ = self._bn_bwd("backbone.bn1", g_a0, None, h(St["a0"]), h(St["u0"]), relu_from_u=True, mask=St["m0"])
+        du0, _ = self._bn_bwd("backbone.bn1", g_a0, None, h(St["u0"]), mask=St["m0"])
         def stem_wgrad():  # on the side stream like every conv wgrad: the split-K workspace is owned by that stream by now
             buf, ks, kss = ops.gemm_wgrad(du0.view(B * 128 * 128, 64), h(St["a_col"]), self.ws)
             # ws rows [64][192] with k = (r*7+s)*3 + c  ->  OIHW [64][3][7][7]
@@ -862,31 +774,51 @@ class Engine:
         return out
 
 
-def out_trans_first(t):
-    return t[0]
-
-
-def _bn_snapshot(engine: "Engine"):
-    """BatchNorm running statistics + counters (graph warm-up iterations must not advance them, ADVICE r1)."""
-    return [(m, m.running_mean.clone(), m.running_var.clone(),
-             None if m.num_batches_tracked is None else m.num_batches_tracked.clone()) for m in engine._bn_mods.values()]
-
-
-def _bn_restore(snap):
-    with torch.no_grad():
-        for m, rm, rv, nbt in snap:
-            m.running_mean.copy_(rm)
-            m.running_var.copy_(rv)
-            if nbt is not None:
-                m.num_batches_tracked.copy_(nbt)
-
-
 def _capture_mode():
     # with a process group alive, NCCL's watchdog thread polls CUDA events while we capture: "thread_local" keeps its
     # calls legal (the collectives themselves are captured into the graph on their side stream)
     import torch.distributed as dist
 
     return "thread_local" if (dist.is_available() and dist.is_initialized()) else "global"
+
+
+def _capture(engine: "Engine", steps, warmup: int, restore_bn: bool = False, pool=None):
+    """Runs `warmup` rounds of the callables `steps` on a side stream (this also sizes the split-K workspace and uploads the
+    pack job tables), then captures each step into its own CUDA graph, all in `pool` if one is given.  Returns
+    [(graph, what the step returned)].  restore_bn: the warm-up leaves the BatchNorm running statistics and counters as
+    they were."""
+    bn_bufs = [t for m in engine._bn_mods.values() for t in m.buffers()] if restore_bn else []
+    snap = [t.clone() for t in bn_bufs]
+    side = torch.cuda.Stream()
+    side.wait_stream(torch.cuda.current_stream())
+    with torch.cuda.stream(side):
+        for _ in range(warmup):
+            for step in steps:
+                step()
+    torch.cuda.current_stream().wait_stream(side)
+    torch.cuda.synchronize()
+    for t, s in zip(bn_bufs, snap):
+        t.copy_(s)
+    out = []
+    for step in steps:
+        graph = torch.cuda.CUDAGraph()
+        with torch.cuda.graph(graph, pool=pool, capture_error_mode=_capture_mode()):
+            out.append((graph, step()))
+    return out
+
+
+def _clone_inputs(x: torch.Tensor, aux: dict):
+    """Static input buffers of a captured graph: clones of x and of the tensors in aux (other entries are shared)."""
+    return x.clone(), {k: (v.clone() if isinstance(v, torch.Tensor) else v) for k, v in aux.items()}
+
+
+def _copy_inputs(static_x: torch.Tensor, static_aux: dict, x: Optional[torch.Tensor], aux: dict):
+    """Copies new inputs into the static buffers (device-side, ordered before the next replay); x = None keeps the old x."""
+    if x is not None:
+        static_x.copy_(x, non_blocking=True)
+    for k, v in aux.items():
+        if isinstance(v, torch.Tensor):
+            static_aux[k].copy_(v, non_blocking=True)
 
 
 def _finish_hook(engine: "Engine"):
@@ -904,8 +836,7 @@ class GraphedTrainStep:
 
     def __init__(self, engine: "Engine", x: torch.Tensor, aux: dict, train_bn: bool = True, warmup: int = 2, after_backward=None):
         self.engine = engine
-        self.x = x.clone()
-        self.aux = {k: (v.clone() if isinstance(v, torch.Tensor) else v) for k, v in aux.items()}
+        self.x, self.aux = _clone_inputs(x, aux)
         if self.aux.get("sym_infos") is not None:  # symmetric PM: only the (first row, count) pairs are a per-step input
             self.aux["sym_idx"] = engine.sym_table.indices(self.aux["sym_infos"])
         self.aux.pop("sym_infos", None)
@@ -919,30 +850,14 @@ class GraphedTrainStep:
                 after_backward()
             return res
 
-        snap = _bn_snapshot(engine)
-        side = torch.cuda.Stream()
-        side.wait_stream(torch.cuda.current_stream())
-        with torch.cuda.stream(side):
-            for _ in range(warmup):  # also sizes the split-K workspace and uploads the pack job table
-                one_step()
-        torch.cuda.current_stream().wait_stream(side)
-        torch.cuda.synchronize()
-        _bn_restore(snap)
-        self.graph = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(self.graph, capture_error_mode=_capture_mode()):
-            res = one_step()
+        [(self.graph, res)] = _capture(engine, [one_step], warmup, restore_bn=True)
         self.losses, self.vis, self.rot, self.trans = res["losses"], res["vis"], res["rot"], res["trans"]
         self.logits = res["logits"]
 
     def __call__(self, x: Optional[torch.Tensor] = None, aux: Optional[dict] = None, grad_losses: Optional[torch.Tensor] = None):
-        if x is not None:
-            self.x.copy_(x, non_blocking=True)
-        if aux is not None:
-            if aux.get("sym_infos") is not None:
-                self.aux["sym_idx"].copy_(self.engine.sym_table.indices(aux["sym_infos"]), non_blocking=True)
-            for k, v in aux.items():
-                if isinstance(v, torch.Tensor):
-                    self.aux[k].copy_(v, non_blocking=True)
+        if aux is not None and aux.get("sym_infos") is not None:
+            self.aux["sym_idx"].copy_(self.engine.sym_table.indices(aux["sym_infos"]), non_blocking=True)
+        _copy_inputs(self.x, self.aux, x, aux or {})
         if grad_losses is not None:
             self.gw.copy_(grad_losses)
         self.graph.replay()
@@ -956,30 +871,18 @@ class GraphedFwdBwd:
 
     def __init__(self, engine: "Engine", x: torch.Tensor, aux: dict, train_bn: bool):
         self.engine, self.train_bn = engine, train_bn
-        self.x = x.clone()
-        self.aux = {k: (v.clone() if isinstance(v, torch.Tensor) else v) for k, v in aux.items()}
+        self.x, self.aux = _clone_inputs(x, aux)
         self.gw = torch.ones(8, device=x.device)
         self.key = self.signature(x, aux, train_bn)
-        snap = _bn_snapshot(engine)
-        side = torch.cuda.Stream()
-        side.wait_stream(torch.cuda.current_stream())
-        with torch.cuda.stream(side), torch.no_grad():
-            for _ in range(2):
-                engine.forward(self.x, self.aux, train_bn=train_bn, do_loss=True)
-                engine.backward(self.gw)
-                _finish_hook(engine)
-        torch.cuda.current_stream().wait_stream(side)
-        torch.cuda.synchronize()
-        _bn_restore(snap)
-        self.g_fwd, self.g_bwd = torch.cuda.CUDAGraph(), torch.cuda.CUDAGraph()
-        pool = torch.cuda.graph_pool_handle()
-        mode = _capture_mode()
+
+        def bwd():
+            engine.backward(self.gw)
+            _finish_hook(engine)
+
         with torch.no_grad():
-            with torch.cuda.graph(self.g_fwd, pool=pool, capture_error_mode=mode):
-                res = engine.forward(self.x, self.aux, train_bn=train_bn, do_loss=True)
-            with torch.cuda.graph(self.g_bwd, pool=pool, capture_error_mode=mode):
-                engine.backward(self.gw)
-                _finish_hook(engine)
+            (self.g_fwd, res), (self.g_bwd, _) = _capture(
+                engine, [lambda: engine.forward(self.x, self.aux, train_bn=train_bn, do_loss=True), bwd], warmup=2,
+                restore_bn=True, pool=torch.cuda.graph_pool_handle())
         self.losses, self.vis = res["losses"], res["vis"]
 
     @staticmethod
@@ -987,10 +890,7 @@ class GraphedFwdBwd:
         return (tuple(x.shape), train_bn, tuple(sorted((k, tuple(v.shape)) for k, v in aux.items() if isinstance(v, torch.Tensor))))
 
     def forward(self, x, aux):
-        self.x.copy_(x, non_blocking=True)
-        for k, v in aux.items():
-            if isinstance(v, torch.Tensor):
-                self.aux[k].copy_(v, non_blocking=True)
+        _copy_inputs(self.x, self.aux, x, aux)
         self.g_fwd.replay()
         return self.losses.clone(), self.vis.clone()
 
@@ -1028,9 +928,7 @@ class _GDRNFunction(torch.autograd.Function):
             ctx.graphed.backward(g_losses)
         else:
             engine.backward(g_losses)
-        hook = engine.grad_hook
-        if hook is not None and hasattr(hook, "finish"):
-            hook.finish()  # the gradients handed to autograd are the all-reduced ones (stream-ordered wait, no host sync)
+        _finish_hook(engine)  # the gradients handed to autograd are the all-reduced ones (stream-ordered wait, no host sync)
         # FRESH views of the flat gradient buffer: autograd's AccumulateGrad adopts a uniquely-referenced contiguous gradient
         # without copying, so after `zero_grad(set_to_none=True)` p.grad aliases Engine.flat_grad and the 148 per-parameter
         # clone kernels (0.4 ms per step) disappear.  materialize_aliased_grads() protects gradient accumulation.

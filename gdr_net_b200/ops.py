@@ -143,16 +143,16 @@ def pack_conv_dgrad(w: torch.Tensor, planes: int, out: PT | None = None) -> PT:
     return out
 
 
-def pack_deconv_fwd_phases(wt: torch.Tensor, planes: int, out: PT | None = None) -> PT:
-    """ConvTranspose2d IOHW [Cin][Cout][k][k] -> the operand of gdrn_conv_dgrad_s2 (rows = Cout, cols = taps x Cin, flipped taps):
-    the transposed conv's forward IS the data gradient of the stride-2 conv whose OIHW weight this tensor is, evaluated by output
-    parity over the un-dilated input (no zero-inserted tensor, 1/4 of the MACs)."""
-    return pack_conv_dgrad(wt, planes, out=out)
+def pack_stem(w: torch.Tensor, planes: int, out: PT | None = None) -> PT:
+    """7x7 stem weight [64][3][7][7] -> [64][192] with k = (r*7+s)*3 + c (matches gdrn_stem_im2col); cols 147..191 stay zero."""
+    out = out or PT((64, 192), planes, device=w.device, zero=True)
+    _pack(w, out, 64, 3, 7, 7, 64, 3, 192, 147, 49, 7, 1, 0)
+    return out
 
 
 def pack_deconv_fwd(wt: torch.Tensor, planes: int, out: PT | None = None) -> PT:
     """ConvTranspose2d IOHW [Cin][Cout][k][k] -> equivalent stride-1 conv over the zero-inserted input
-    (taps flipped): rows = Cout, cols = Cin.  (First formulation, kept for the op tests / A-B.)"""
+    (taps flipped): rows = Cout, cols = Cin.  (First formulation, kept for the op tests.)"""
     I, O, KH, KW = wt.shape
     opad, ipad = _round_up(O, 64), _round_up(I, 64)
     krow = KH * KW * ipad

@@ -20,6 +20,29 @@ from .capi import C
 from .ops import PT, _stream
 
 
+def pnp_net_forward(x: PT, net, wf: dict, b_rt: torch.Tensor, pred: torch.Tensor, saved: list | None = None):
+    """3 x (conv 3x3 s2 -> GroupNorm + ReLU) -> fc1 -> fc2 -> fc_r|fc_t of `net` (a ConvPnPNet) on the 128-channel input
+    planes x [B, 64, 64, 128].  wf: packed operands "pnp_net.features.{0,3,6}" (pack_conv_fwd), "fc1", "fc2" and "fc_rt"
+    (pack_linear of fc_r and fc_t stacked), b_rt their stacked bias.  pred [B, 16] fp32 receives rot in its first
+    fc_r.out_features columns and t in the next 3.  saved: receives dict(ci, gi, x_in, u, y, gstats) per conv for backward.
+    Returns the inputs of fc1, fc2 and fc_r|fc_t."""
+    B = x.shape[0]
+    cur = x
+    for ci, gi in ((0, 1), (3, 4), (6, 7)):
+        gn = net.features[gi]
+        u = ops.conv_fwd(cur, wf[f"pnp_net.features.{ci}"], 128, 3, 3, 2, 1)
+        gstats = torch.empty(B, 32, 2, device=pred.device)
+        y = ops.gn_relu_fwd(u, gn.weight, gn.bias, gstats, G=gn.num_groups, eps=gn.eps)
+        if saved is not None:
+            saved.append(dict(ci=ci, gi=gi, x_in=cur, u=u, y=y, gstats=gstats))
+        cur = y
+    flat = cur.view(B, 8192)
+    h1 = ops.gemm_fwd(flat, wf["fc1"], 1024, bias=net.fc1.bias, act=1)
+    h2 = ops.gemm_fwd(h1, wf["fc2"], 256, bias=net.fc2.bias, act=1)
+    ops.gemm_fwd(h2, wf["fc_rt"], net.fc_r.out_features + 3, out_f32=pred, bias=b_rt, ldc=16, want_planes=False)
+    return flat, h1, h2
+
+
 class PatchPnP:
     def __init__(self, pnp_net, precision: str = "fp32x3"):
         precision = {"mixed": "fp32x3", "fp16": "half", "bf16": "half"}.get(precision, precision)
@@ -42,7 +65,8 @@ class PatchPnP:
         pl, wf = self.planes, self.wf
         dev = n.fc1.weight.device
         for ci in (0, 3, 6):
-            wf[ci] = ops.pack_conv_fwd(n.features[ci].weight.detach(), pl, out=wf.get(ci), ipad=128)
+            k = f"pnp_net.features.{ci}"
+            wf[k] = ops.pack_conv_fwd(n.features[ci].weight.detach(), pl, out=wf.get(k), ipad=128)
         wf["fc1"] = ops.pack_linear(n.fc1.weight.detach(), pl, out=wf.get("fc1"), nhwc_from=(128, 8, 8))
         wf["fc2"] = ops.pack_linear(n.fc2.weight.detach(), pl, out=wf.get("fc2"))
         if "w_rt" not in wf:
@@ -57,21 +81,12 @@ class PatchPnP:
 
     # ------------------------------------------------------------------ the kernel sequence
     def _run(self, coor_feat, region, extents, pred):
-        n, pl = self.net, self.planes
         B, c_feat = coor_feat.shape[0], coor_feat.shape[1]
         c_reg = 0 if region is None else region.shape[1]
-        x = PT((B, 64, 64, 128), pl, device=coor_feat.device)
+        x = PT((B, 64, 64, 128), self.planes, device=coor_feat.device)
         C.gdrn_pnp_pack_input(coor_feat.data_ptr(), c_feat, ops.ptr(region), c_reg, ops.ptr(extents), x.hi_ptr, x.lo_ptr, B, 4096,
                               _stream())
-        cur = x
-        for ci, gi in ((0, 1), (3, 4), (6, 7)):
-            u = ops.conv_fwd(cur, self.wf[ci], 128, 3, 3, 2, 1)
-            gstats = torch.empty(B, 32, 2, device=coor_feat.device)
-            cur = ops.gn_relu_fwd(u, n.features[gi].weight, n.features[gi].bias, gstats, G=n.features[gi].num_groups,
-                                  eps=n.features[gi].eps)
-        h1 = ops.gemm_fwd(cur.view(B, 8192), self.wf["fc1"], 1024, bias=n.fc1.bias, act=1)
-        h2 = ops.gemm_fwd(h1, self.wf["fc2"], 256, bias=n.fc2.bias, act=1)
-        ops.gemm_fwd(h2, self.wf["fc_rt"], n.fc_r.out_features + 3, out_f32=pred, bias=self.wf["b_rt"], ldc=16, want_planes=False)
+        pnp_net_forward(x, self.net, self.wf, self.wf["b_rt"], pred)
 
     @torch.no_grad()
     def __call__(self, coor_feat: torch.Tensor, region: torch.Tensor | None = None, extents: torch.Tensor | None = None):
