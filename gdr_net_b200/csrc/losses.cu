@@ -45,6 +45,11 @@ __device__ __forceinline__ void load_logits(const float* __restrict__ logits, lo
     }
 }
 
+// a * w - b * w with both products rounded, like the reference's l1_loss(a * w, b * w): exactly 0 when a == b, so the L1
+// gradient sign(0) = 0 there.  Without __fmul_rn the compiler contracts it to fma(a, w, -(b * w)), which leaves the rounding
+// error of b * w and turns that 0 into a +-1 of arbitrary sign.
+__device__ __forceinline__ float masked_diff(float a, float b, float w) { return __fmul_rn(a, w) - __fmul_rn(b, w); }
+
 // ------------------------------------------------------------------------------------------------
 // W2D: the Patch-PnP input carries the 2-D crop coordinates (cfg PNP_NET.WITH_2D_COORD: 3 + 2 + 64 = 69 channels, region at
 // 5..68) or not (3 + 64 = 67 channels, region at 3..66) -- GDRN.py:171-173, :635-647
@@ -138,7 +143,7 @@ __global__ void __launch_bounds__(128) pixel_loss_fwd_kernel(const float* __rest
         load_logits(logits, pix, z);
         const float mv = __ldg(m_visib + pix), mt = __ldg(m_trunc + pix);
 #pragma unroll
-        for (int j = 0; j < 3; ++j) acc[j] += fabsf(z[1 + j] * mv - __ldg(gt_xyz + ((long)b * 3 + j) * HW + hw) * mv);
+        for (int j = 0; j < 3; ++j) acc[j] += fabsf(masked_diff(z[1 + j], __ldg(gt_xyz + ((long)b * 3 + j) * HW + hw), mv));
         acc[3] += fabsf(z[0] - mt);
         // CE over 65 logits (bg + 64), logits and label multiplied by the visible mask
         float mx = -INFINITY;
@@ -223,7 +228,7 @@ __global__ void __launch_bounds__(128) head_bwd_kernel(const float* __restrict__
         const float gws[3] = {gwx, gwy, gwz};
 #pragma unroll
         for (int j = 0; j < 3; ++j) {
-            const float e = z[1 + j] * mv - __ldg(gt_xyz + ((long)b * 3 + j) * HW + hw) * mv;
+            const float e = masked_diff(z[1 + j], __ldg(gt_xyz + ((long)b * 3 + j) * HW + hw), mv);
             const float sg = e > 0.f ? 1.f : (e < 0.f ? -1.f : 0.f);
             d[1 + j] = gws[j] * inv_fg * sg * mv + gin[j] * __ldg(extents + b * 3 + j);
         }
@@ -583,7 +588,7 @@ __global__ void __launch_bounds__(128) pose_loss_kernel(const PoseParams p) {
             // reference computes est and tgt separately then subtracts; (R - Rgt) p is the same up to rounding
             const float est = sR[i * 3] * px + sR[i * 3 + 1] * py + sR[i * 3 + 2] * pz;
             const float tgt = sRgt[i * 3] * px + sRgt[i * 3 + 1] * py + sRgt[i * 3 + 2] * pz;
-            const float e = w * est - w * tgt;
+            const float e = masked_diff(est, tgt, w);
             acc += fabsf(e);
             const float sg = e > 0.f ? w : (e < 0.f ? -w : 0.f);
             G[i * 3] += sg * px;
