@@ -195,10 +195,12 @@ def _check_supported(cfg):
         problems.append("backbone must be resnet18/34 at 256 -> 64")
     if r.ROT_CONCAT or r.ROT_CLASS_AWARE or r.MASK_CLASS_AWARE or r.REGION_CLASS_AWARE:
         problems.append("class-aware / concat heads")
-    if r.XYZ_LOSS_TYPE != "L1" or r.MASK_LOSS_TYPE != "L1" or r.REGION_LOSS_TYPE != "CE" or r.NUM_REGIONS != 64:
-        problems.append("losses other than xyz L1 / mask L1 / region CE over 64 regions")
-    if r.XYZ_LOSS_MASK_GT != "visib" or r.MASK_LOSS_GT != "trunc" or r.REGION_LOSS_MASK_GT != "visib":
-        problems.append("mask selection other than visib/trunc/visib")
+    if r.XYZ_LOSS_TYPE != "L1" or r.MASK_LOSS_TYPE not in ("L1", "BCE", "CE") or r.REGION_LOSS_TYPE != "CE" or r.NUM_REGIONS != 64:
+        problems.append("losses other than xyz L1 / mask L1, BCE or CE / region CE over 64 regions")
+    # gdrn_loss builds gt_masks = {"trunc", "visib", "obj"} (GDRN.py:339); any other key (the config comment's "gt") is a KeyError there
+    for key in ("XYZ_LOSS_MASK_GT", "MASK_LOSS_GT", "REGION_LOSS_MASK_GT"):
+        if getattr(r, key) not in ("trunc", "visib", "obj"):
+            problems.append(f"ROT_HEAD.{key} = {getattr(r, key)!r} (trunc, visib or obj)")
     if not p.REGION_ATTENTION or p.MASK_ATTENTION != "none" or p.R_ONLY:
         problems.append("Patch-PnP input other than xyz (+ 2D coords) + region attention")
     if p.ROT_TYPE != "allo_rot6d" or p.TRANS_TYPE != "centroid_z" or p.Z_TYPE != "REL":
@@ -268,7 +270,7 @@ class GDRN(nn.Module):
         res = self.engine.run(
             x, roi_coord_2d=roi_coord_2d, roi_cams=roi_cams, roi_centers=roi_centers, roi_whs=roi_whs,
             roi_extents=roi_extents, resize_ratios=resize_ratios, gt_xyz=gt_xyz, gt_mask_trunc=gt_mask_trunc,
-            gt_mask_visib=gt_mask_visib, gt_region=gt_region, gt_ego_rot=gt_ego_rot, gt_points=gt_points,
+            gt_mask_visib=gt_mask_visib, gt_mask_obj=gt_mask_obj, gt_region=gt_region, gt_ego_rot=gt_ego_rot, gt_points=gt_points,
             sym_infos=sym_infos if pnp_cfg.PM_LOSS_SYM else None, gt_trans=gt_trans, gt_trans_ratio=gt_trans_ratio,
             do_loss=do_loss, train_bn=self.training, want_maps=(not do_loss) and bool(cfg.TEST.USE_PNP),
         )

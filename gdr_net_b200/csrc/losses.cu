@@ -2,7 +2,8 @@
 //
 //   head_glue_fwd   GDRN.py:156-169 + conv_pnp_net.py:120-125: softmax(region[:,1:]), cat(xyz, coord2d, region),
 //                   (xyz-0.5)*extent  -> NHWC bf16 Patch-PnP input (69 valid of 128 channels)
-//   pixel_loss_fwd  GDRN.py:341-400: masked L1 on x,y,z, L1-mean on mask, CE-sum on region (SURVEY P5 quirk)
+//   pixel_loss_fwd  GDRN.py:341-400: masked L1 on x,y,z, L1 / BCE / 2-class CE mean on mask, CE-sum on region (SURVEY P5
+//                   quirk); each of the three takes its own GT mask (XYZ_LOSS_MASK_GT, MASK_LOSS_GT, REGION_LOSS_MASK_GT)
 //   head_bwd        analytic backward of both of the above, fused: one pass over the logits
 //   pose_loss       rot_reps.py:34-49, pose_from_pred_centroid_z.py:144-227, utils.py:208-236,
 //                   pose_utils.py:323-370 (quat2mat), pm_loss.py:82-114, pose_utils.py:430-482 (closest
@@ -16,9 +17,44 @@
 namespace gdrn {
 
 typedef __nv_bfloat16 bf16;
-constexpr int kLogitLd = 72;   // 69 logits padded to 72 floats per pixel
+constexpr int kLogitLd = 72;   // 68 + MO logits padded to 72 floats per pixel
 constexpr int kPnpLd = 128;    // Patch-PnP input channels padded to 128
 constexpr int kNumReg = 64;    // foreground regions (region logits: bg + 64)
+
+// Mask head (ROT_HEAD.MASK_LOSS_TYPE, GDRN.py:376-385): MO = 1 mask logit for L1 and BCE, MO = 2 for CE.  A logit row is
+// mask [0, MO) | xyz [MO, MO + 3) | bg MO + 3 | regions [MO + 4, MO + 68)  (cdpn_rot_head_region.py:185-192).
+enum MaskLoss { kMaskL1 = 0, kMaskBCE = 1, kMaskCE = 2 };
+
+// Per-pixel mask loss against the target t (GT mask value): |z - t|; BCEWithLogits in the stable form
+// max(z, 0) - z t + log1p(exp(-|z|)); CrossEntropy over (z0, z1) with label (int) t, the reference's .long() truncation.
+template <int MODE>
+__device__ __forceinline__ float mask_loss(const float (&z)[kLogitLd], float t) {
+    if (MODE == kMaskL1) return fabsf(z[0] - t);
+    if (MODE == kMaskBCE) return fmaxf(z[0], 0.f) - z[0] * t + log1pf(expf(-fabsf(z[0])));
+    const float lse = fmaxf(z[0], z[1]) + log1pf(expf(-fabsf(z[0] - z[1])));
+    return lse - ((int)t == 1 ? z[1] : z[0]);
+}
+
+// logistic sigmoid without overflow: exp of a non-positive argument only
+__device__ __forceinline__ float sigmoid_stable(float x) {
+    const float e = expf(-fabsf(x));
+    return x >= 0.f ? 1.f / (1.f + e) : e / (1.f + e);
+}
+
+// d(mask loss)/d(mask logits) scaled by c = upstream gradient / (B HW): sign(z - t); sigmoid(z) - t; softmax - onehot
+template <int MODE>
+__device__ __forceinline__ void mask_loss_bwd(const float (&z)[kLogitLd], float t, float c, float (&d)[72]) {
+    if (MODE == kMaskL1) {
+        const float e = z[0] - t;
+        d[0] = c * (e > 0.f ? 1.f : (e < 0.f ? -1.f : 0.f));
+    } else if (MODE == kMaskBCE) {
+        d[0] = c * (sigmoid_stable(z[0]) - t);
+    } else {
+        const int lab = (int)t;
+        d[0] = c * (sigmoid_stable(z[0] - z[1]) - (lab == 1 ? 0.f : 1.f));
+        d[1] = c * (sigmoid_stable(z[1] - z[0]) - (lab == 1 ? 1.f : 0.f));
+    }
+}
 
 __device__ __forceinline__ void store_row_bf16(bf16* hi, bf16* lo, long row, int ld, const float* v, int n) {
     // n multiple of 8, v[n] in registers/local
@@ -53,7 +89,7 @@ __device__ __forceinline__ float masked_diff(float a, float b, float w) { return
 // ------------------------------------------------------------------------------------------------
 // W2D: the Patch-PnP input carries the 2-D crop coordinates (cfg PNP_NET.WITH_2D_COORD: 3 + 2 + 64 = 69 channels, region at
 // 5..68) or not (3 + 64 = 67 channels, region at 3..66) -- GDRN.py:171-173, :635-647
-template <bool W2D>
+template <int MO, bool W2D>
 __global__ void __launch_bounds__(128) head_glue_fwd_kernel(const float* __restrict__ logits, const float* __restrict__ coord2d,
                                                             const float* __restrict__ extents, bf16* __restrict__ out_hi,
                                                             bf16* __restrict__ out_lo, int B, int HW) {
@@ -65,7 +101,7 @@ __global__ void __launch_bounds__(128) head_glue_fwd_kernel(const float* __restr
         load_logits(logits, pix, z);
         float o[72];
 #pragma unroll
-        for (int j = 0; j < 3; ++j) o[j] = (z[1 + j] - 0.5f) * __ldg(extents + b * 3 + j);
+        for (int j = 0; j < 3; ++j) o[j] = (z[MO + j] - 0.5f) * __ldg(extents + b * 3 + j);
         constexpr int RO = W2D ? 5 : 3;  // first region channel
         if (W2D) {
             o[3] = __ldg(coord2d + ((long)b * 2 + 0) * HW + hw);
@@ -73,11 +109,11 @@ __global__ void __launch_bounds__(128) head_glue_fwd_kernel(const float* __restr
         }
         float m = -INFINITY;
 #pragma unroll
-        for (int k = 0; k < kNumReg; ++k) m = fmaxf(m, z[5 + k]);
+        for (int k = 0; k < kNumReg; ++k) m = fmaxf(m, z[MO + 4 + k]);
         float s = 0.f;
 #pragma unroll
         for (int k = 0; k < kNumReg; ++k) {
-            o[RO + k] = expf(z[5 + k] - m);
+            o[RO + k] = expf(z[MO + 4 + k] - m);
             s += o[RO + k];
         }
         const float inv = 1.f / s;
@@ -129,61 +165,73 @@ __global__ void __launch_bounds__(128) pnp_pack_input_kernel(const float* __rest
     }
 }
 
-// sums (double[6]): |dx|, |dy|, |dz| (masked), |mask - trunc|, CE, sum(mask_visib)
+// sums (double[7]): |dx|, |dy|, |dz| (masked), mask loss, region CE, sum(xyz mask), sum(region mask).  SEP = the region mask
+// is not the xyz mask; without it the region terms reuse the xyz mask and slot 6 gets slot 5's partials.  n_sums = 6 writes
+// slots 0..5 only (the original six-slot layout; needs !SEP).
+template <int MODE, int MO, bool SEP>
 __global__ void __launch_bounds__(128) pixel_loss_fwd_kernel(const float* __restrict__ logits, const float* __restrict__ gt_xyz,
-                                                             const float* __restrict__ m_visib, const float* __restrict__ m_trunc,
-                                                             const long long* __restrict__ labels, double* __restrict__ sums,
-                                                             int B, int HW) {
+                                                             const float* __restrict__ m_xyz, const float* __restrict__ m_tgt,
+                                                             const float* __restrict__ m_reg, const long long* __restrict__ labels,
+                                                             double* __restrict__ sums, int n_sums, int B, int HW) {
+    constexpr int NACC = SEP ? 7 : 6;
     const long total = (long)B * HW;
-    float acc[6] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+    float acc[NACC];
+#pragma unroll
+    for (int j = 0; j < NACC; ++j) acc[j] = 0.f;
     for (long pix = blockIdx.x * (long)blockDim.x + threadIdx.x; pix < total; pix += (long)gridDim.x * blockDim.x) {
         const int b = (int)(pix / HW);
         const int hw = (int)(pix - (long)b * HW);
         float z[kLogitLd];
         load_logits(logits, pix, z);
-        const float mv = __ldg(m_visib + pix), mt = __ldg(m_trunc + pix);
+        const float mv = __ldg(m_xyz + pix), mt = __ldg(m_tgt + pix);
+        const float mr = SEP ? __ldg(m_reg + pix) : mv;
 #pragma unroll
-        for (int j = 0; j < 3; ++j) acc[j] += fabsf(masked_diff(z[1 + j], __ldg(gt_xyz + ((long)b * 3 + j) * HW + hw), mv));
-        acc[3] += fabsf(z[0] - mt);
-        // CE over 65 logits (bg + 64), logits and label multiplied by the visible mask
+        for (int j = 0; j < 3; ++j) acc[j] += fabsf(masked_diff(z[MO + j], __ldg(gt_xyz + ((long)b * 3 + j) * HW + hw), mv));
+        acc[3] += mask_loss<MODE>(z, mt);
+        // CE over 65 logits (bg + 64), logits and label multiplied by the region mask
         float mx = -INFINITY;
 #pragma unroll
-        for (int k = 0; k < 65; ++k) mx = fmaxf(mx, z[4 + k] * mv);
+        for (int k = 0; k < 65; ++k) mx = fmaxf(mx, z[MO + 3 + k] * mr);
         float s = 0.f;
 #pragma unroll
-        for (int k = 0; k < 65; ++k) s += expf(z[4 + k] * mv - mx);
-        const int lab = (int)(__ldg(labels + pix) * (long long)mv);
+        for (int k = 0; k < 65; ++k) s += expf(z[MO + 3 + k] * mr - mx);
+        const int lab = (int)(__ldg(labels + pix) * (long long)mr);
         float zl = 0.f;
 #pragma unroll
-        for (int k = 0; k < 65; ++k) zl = (k == lab) ? z[4 + k] * mv : zl;
+        for (int k = 0; k < 65; ++k) zl = (k == lab) ? z[MO + 3 + k] * mr : zl;
         acc[4] += (logf(s) + mx) - zl;
         acc[5] += mv;
+        if (SEP) acc[NACC - 1] += mr;
     }
-    __shared__ float red[6][4];
+    __shared__ float red[NACC][4];
 #pragma unroll
-    for (int j = 0; j < 6; ++j) {
+    for (int j = 0; j < NACC; ++j) {
         float v = acc[j];
         for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
         if ((threadIdx.x & 31) == 0) red[j][threadIdx.x >> 5] = v;
     }
     __syncthreads();
-    if (threadIdx.x < 6) {
-        const float v = red[threadIdx.x][0] + red[threadIdx.x][1] + red[threadIdx.x][2] + red[threadIdx.x][3];
+    if (threadIdx.x < n_sums) {
+        const int j = threadIdx.x < NACC ? threadIdx.x : 5;
+        const float v = red[j][0] + red[j][1] + red[j][2] + red[j][3];
         atomicAdd(sums + threadIdx.x, (double)v);
     }
 }
 
-// d_logits (bf16 hi/lo, [P][128], cols >= 69 zero) = d(pixel losses) + glue backward of d_pnp_in
-// gw[5]: upstream gradients of loss_coor_x, _y, _z, loss_mask, loss_region
-template <bool W2D>
+// d_logits (bf16 hi/lo, [P][128], cols >= 68 + MO zero) = d(pixel losses) + glue backward of d_pnp_in
+// gw[5]: upstream gradients of loss_coor_x, _y, _z, loss_mask, loss_region.  Normalisers: sums[5] (xyz), sums[6] (region, SEP
+// only: without SEP the region mask is the xyz mask and slot 6 is not read).
+template <int MODE, int MO, bool SEP, bool W2D>
 __global__ void __launch_bounds__(128) head_bwd_kernel(const float* __restrict__ logits, const float* __restrict__ gt_xyz,
-                                                       const float* __restrict__ m_visib, const float* __restrict__ m_trunc,
-                                                       const long long* __restrict__ labels, const double* __restrict__ sums,
+                                                       const float* __restrict__ m_xyz, const float* __restrict__ m_tgt,
+                                                       const float* __restrict__ m_reg, const long long* __restrict__ labels,
+                                                       const double* __restrict__ sums,
                                                        const float* __restrict__ gw, const bf16* __restrict__ din_hi,
                                                        const bf16* __restrict__ din_lo, const float* __restrict__ extents,
                                                        bf16* __restrict__ out_hi, bf16* __restrict__ out_lo, int B, int HW) {
     const long total = (long)B * HW;
     const float inv_fg = 1.f / fmaxf((float)sums[5], 1.f);
+    const float inv_reg = SEP ? 1.f / fmaxf((float)sums[6], 1.f) : inv_fg;
     const float inv_all = 1.f / (float)total;
     const float gwx = gw[0], gwy = gw[1], gwz = gw[2], gwm = gw[3], gwr = gw[4];
     for (long pix = blockIdx.x * (long)blockDim.x + threadIdx.x; pix < total; pix += (long)gridDim.x * blockDim.x) {
@@ -191,13 +239,11 @@ __global__ void __launch_bounds__(128) head_bwd_kernel(const float* __restrict__
         const int hw = (int)(pix - (long)b * HW);
         float z[kLogitLd];
         load_logits(logits, pix, z);
-        const float mv = __ldg(m_visib + pix), mt = __ldg(m_trunc + pix);
+        const float mv = __ldg(m_xyz + pix), mt = __ldg(m_tgt + pix);
+        const float mr = SEP ? __ldg(m_reg + pix) : mv;
         float d[72];
-        // mask channel: L1 mean
-        {
-            const float e = z[0] - mt;
-            d[0] = gwm * inv_all * (e > 0.f ? 1.f : (e < 0.f ? -1.f : 0.f));
-        }
+        // mask channels: mean over B HW pixels
+        mask_loss_bwd<MODE>(z, mt, gwm * inv_all, d);
         // Patch-PnP input gradient (hi+lo)
         float gin[72];
         if (din_hi != nullptr) {
@@ -228,38 +274,38 @@ __global__ void __launch_bounds__(128) head_bwd_kernel(const float* __restrict__
         const float gws[3] = {gwx, gwy, gwz};
 #pragma unroll
         for (int j = 0; j < 3; ++j) {
-            const float e = masked_diff(z[1 + j], __ldg(gt_xyz + ((long)b * 3 + j) * HW + hw), mv);
+            const float e = masked_diff(z[MO + j], __ldg(gt_xyz + ((long)b * 3 + j) * HW + hw), mv);
             const float sg = e > 0.f ? 1.f : (e < 0.f ? -1.f : 0.f);
-            d[1 + j] = gws[j] * inv_fg * sg * mv + gin[j] * __ldg(extents + b * 3 + j);
+            d[MO + j] = gws[j] * inv_fg * sg * mv + gin[j] * __ldg(extents + b * 3 + j);
         }
         // region CE over 65 (masked logits): d = m * (softmax65(z*m) - onehot(label*m)) / max(sum m, 1)
         {
             float mx = -INFINITY;
 #pragma unroll
-            for (int k = 0; k < 65; ++k) mx = fmaxf(mx, z[4 + k] * mv);
+            for (int k = 0; k < 65; ++k) mx = fmaxf(mx, z[MO + 3 + k] * mr);
             float s = 0.f;
 #pragma unroll
             for (int k = 0; k < 65; ++k) {
-                d[4 + k] = expf(z[4 + k] * mv - mx);
-                s += d[4 + k];
+                d[MO + 3 + k] = expf(z[MO + 3 + k] * mr - mx);
+                s += d[MO + 3 + k];
             }
-            const float c = gwr * inv_fg * mv;
+            const float c = gwr * inv_reg * mr;
             const float inv = 1.f / s;
-            const int lab = (int)(__ldg(labels + pix) * (long long)mv);
+            const int lab = (int)(__ldg(labels + pix) * (long long)mr);
 #pragma unroll
-            for (int k = 0; k < 65; ++k) d[4 + k] = c * (d[4 + k] * inv - (k == lab ? 1.f : 0.f));
+            for (int k = 0; k < 65; ++k) d[MO + 3 + k] = c * (d[MO + 3 + k] * inv - (k == lab ? 1.f : 0.f));
         }
         // softmax64 backward of the Patch-PnP region-attention input: dz_k = p_k (g_k - sum_j g_j p_j)
         if (din_hi != nullptr) {
             constexpr int RO = W2D ? 5 : 3;  // first region channel of the Patch-PnP input
             float mx = -INFINITY;
 #pragma unroll
-            for (int k = 0; k < kNumReg; ++k) mx = fmaxf(mx, z[5 + k]);
+            for (int k = 0; k < kNumReg; ++k) mx = fmaxf(mx, z[MO + 4 + k]);
             float s = 0.f, dot = 0.f;
             float pk[kNumReg];
 #pragma unroll
             for (int k = 0; k < kNumReg; ++k) {
-                pk[k] = expf(z[5 + k] - mx);
+                pk[k] = expf(z[MO + 4 + k] - mx);
                 s += pk[k];
             }
             const float inv = 1.f / s;
@@ -269,9 +315,10 @@ __global__ void __launch_bounds__(128) head_bwd_kernel(const float* __restrict__
                 dot = fmaf(gin[RO + k], pk[k], dot);
             }
 #pragma unroll
-            for (int k = 0; k < kNumReg; ++k) d[5 + k] += pk[k] * (gin[RO + k] - dot);
+            for (int k = 0; k < kNumReg; ++k) d[MO + 4 + k] += pk[k] * (gin[RO + k] - dot);
         }
-        d[69] = d[70] = d[71] = 0.f;
+#pragma unroll
+        for (int k = 68 + MO; k < 72; ++k) d[k] = 0.f;
         store_row_bf16(out_hi, out_lo, pix, kPnpLd, d, 72);
         const uint4 zz = make_uint4(0, 0, 0, 0);
         for (int j = 72; j < kPnpLd; j += 8) {
@@ -642,16 +689,18 @@ __global__ void __launch_bounds__(128) pose_loss_kernel(const PoseParams p) {
 }
 
 // losses[8] = coor_x, coor_y, coor_z, mask, region, PM_R, centroid, z ; vis_out[2] = mean re, mean te
+// reg_slot: the pix_sums slot holding sum(region mask), 6, or 5 for the six-slot layout whose region mask is the xyz mask
 __global__ void loss_finalize_kernel(const double* __restrict__ pix_sums, const double* __restrict__ pose_sums,
                                      const float* __restrict__ vis, float* __restrict__ losses, float* __restrict__ vis_out,
-                                     int B, int HW, int n_pts) {
+                                     int B, int HW, int n_pts, int reg_slot) {
     if (threadIdx.x != 0 || blockIdx.x != 0) return;
     const double fg = pix_sums[5] < 1.0 ? 1.0 : pix_sums[5];
+    const double fg_reg = pix_sums[reg_slot] < 1.0 ? 1.0 : pix_sums[reg_slot];
     losses[0] = (float)(pix_sums[0] / fg);
     losses[1] = (float)(pix_sums[1] / fg);
     losses[2] = (float)(pix_sums[2] / fg);
     losses[3] = (float)(pix_sums[3] / ((double)B * HW));
-    losses[4] = (float)(pix_sums[4] / fg);
+    losses[4] = (float)(pix_sums[4] / fg_reg);
     losses[5] = (float)(pose_sums[0] / ((double)B * n_pts));
     losses[6] = (float)(pose_sums[1] / (2.0 * B));
     losses[7] = (float)(pose_sums[2] / (double)B);
@@ -674,17 +723,36 @@ static inline int px_grid(long total) {
     return (int)(g < cap ? (g < 1 ? 1 : g) : cap);
 }
 
-extern "C" int gdrn_head_glue_fwd(const float* logits, const float* coord2d, const float* extents, void* out_hi, void* out_lo,
-                                  int B, int HW, int with_2d, void* stream_) {
+// (mask_loss, mask_out) pairs the head can have: L1 and BCE with one mask logit, CE with two
+static int check_mask_head(const char* fn, int mask_loss, int mask_out) {
+    const bool ok = (mask_loss == kMaskL1 && mask_out == 1) || (mask_loss == kMaskBCE && mask_out == 1) ||
+                    (mask_loss == kMaskCE && mask_out == 2);
+    return ok ? 0 : set_error(GDRN_ERR_ARG, "%s: unsupported mask head (mask_loss %d, mask_out %d)", fn, mask_loss, mask_out);
+}
+
+extern "C" int gdrn_head_glue_fwd_ex(const float* logits, const float* coord2d, const float* extents, void* out_hi, void* out_lo,
+                                     int B, int HW, int with_2d, int mask_out, void* stream_) {
     cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
     if (with_2d && coord2d == nullptr) return set_error(GDRN_ERR_ARG, "head_glue_fwd: with_2d needs coord2d");
-    if (with_2d)
-        head_glue_fwd_kernel<true><<<px_grid((long)B * HW), 128, 0, stream>>>(logits, coord2d, extents, (bf16*)out_hi, (bf16*)out_lo, B, HW);
-    else
-        head_glue_fwd_kernel<false><<<px_grid((long)B * HW), 128, 0, stream>>>(logits, coord2d, extents, (bf16*)out_hi, (bf16*)out_lo, B, HW);
+    if (mask_out != 1 && mask_out != 2) return set_error(GDRN_ERR_ARG, "head_glue_fwd: mask_out %d (1 or 2)", mask_out);
+    const int grid = px_grid((long)B * HW);
+#define GLUE(MO, W2D) head_glue_fwd_kernel<MO, W2D><<<grid, 128, 0, stream>>>(logits, coord2d, extents, (bf16*)out_hi, (bf16*)out_lo, B, HW)
+    if (mask_out == 1) {
+        if (with_2d) GLUE(1, true);
+        else GLUE(1, false);
+    } else {
+        if (with_2d) GLUE(2, true);
+        else GLUE(2, false);
+    }
+#undef GLUE
     GDRN_CUDA_OK(cudaGetLastError());
     count_launch();
     return 0;
+}
+
+extern "C" int gdrn_head_glue_fwd(const float* logits, const float* coord2d, const float* extents, void* out_hi, void* out_lo,
+                                  int B, int HW, int with_2d, void* stream_) {
+    return gdrn_head_glue_fwd_ex(logits, coord2d, extents, out_hi, out_lo, B, HW, with_2d, 1, stream_);
 }
 
 extern "C" int gdrn_pnp_pack_input(const float* coor_feat, int c_feat, const float* region, int c_reg, const float* extents,
@@ -700,11 +768,79 @@ extern "C" int gdrn_pnp_pack_input(const float* coor_feat, int c_feat, const flo
     return 0;
 }
 
+// n_sums 7: the generalised layout; 6: the original one (slot 6 absent, region mask == xyz mask)
+static int pixel_loss_launch(const float* logits, const float* gt_xyz, const float* m_xyz, const float* m_tgt, const float* m_reg,
+                             const long long* labels, double* sums, int n_sums, int B, int HW, int mask_loss, cudaStream_t stream) {
+    GDRN_CUDA_OK(cudaMemsetAsync(sums, 0, n_sums * sizeof(double), stream));
+    const int grid = px_grid((long)B * HW);
+    const bool sep = m_reg != m_xyz;
+#define PIX(MODE, MO, SEP) \
+    pixel_loss_fwd_kernel<MODE, MO, SEP><<<grid, 128, 0, stream>>>(logits, gt_xyz, m_xyz, m_tgt, m_reg, labels, sums, n_sums, B, HW)
+    if (mask_loss == kMaskL1) {
+        if (sep) PIX(kMaskL1, 1, true);
+        else PIX(kMaskL1, 1, false);
+    } else if (mask_loss == kMaskBCE) {
+        if (sep) PIX(kMaskBCE, 1, true);
+        else PIX(kMaskBCE, 1, false);
+    } else {
+        if (sep) PIX(kMaskCE, 2, true);
+        else PIX(kMaskCE, 2, false);
+    }
+#undef PIX
+    GDRN_CUDA_OK(cudaGetLastError());
+    count_launch();
+    return 0;
+}
+
+extern "C" int gdrn_pixel_loss_fwd_ex(const float* logits, const float* gt_xyz, const float* m_xyz, const float* m_mask,
+                                      const float* m_region, const long long* labels, double* sums, int B, int HW, int mask_loss,
+                                      int mask_out, void* stream_) {
+    if (int rc = check_mask_head("pixel_loss_fwd", mask_loss, mask_out)) return rc;
+    return pixel_loss_launch(logits, gt_xyz, m_xyz, m_mask, m_region, labels, sums, 7, B, HW, mask_loss,
+                             reinterpret_cast<cudaStream_t>(stream_));
+}
+
 extern "C" int gdrn_pixel_loss_fwd(const float* logits, const float* gt_xyz, const float* m_visib, const float* m_trunc,
                                    const long long* labels, double* sums, int B, int HW, void* stream_) {
+    return pixel_loss_launch(logits, gt_xyz, m_visib, m_trunc, m_visib, labels, sums, 6, B, HW, kMaskL1,
+                             reinterpret_cast<cudaStream_t>(stream_));
+}
+
+template <int MODE, int MO, bool SEP>
+static void head_bwd_launch(const float* logits, const float* gt_xyz, const float* m_xyz, const float* m_tgt, const float* m_reg,
+                            const long long* labels, const double* sums, const float* gw, const void* din_hi, const void* din_lo,
+                            const float* extents, void* out_hi, void* out_lo, int B, int HW, int with_2d, cudaStream_t stream) {
+    const int grid = px_grid((long)B * HW);
+    if (with_2d)
+        head_bwd_kernel<MODE, MO, SEP, true><<<grid, 128, 0, stream>>>(logits, gt_xyz, m_xyz, m_tgt, m_reg, labels, sums, gw,
+                                                                       (const bf16*)din_hi, (const bf16*)din_lo, extents,
+                                                                       (bf16*)out_hi, (bf16*)out_lo, B, HW);
+    else
+        head_bwd_kernel<MODE, MO, SEP, false><<<grid, 128, 0, stream>>>(logits, gt_xyz, m_xyz, m_tgt, m_reg, labels, sums, gw,
+                                                                        (const bf16*)din_hi, (const bf16*)din_lo, extents,
+                                                                        (bf16*)out_hi, (bf16*)out_lo, B, HW);
+}
+
+extern "C" int gdrn_head_bwd_ex(const float* logits, const float* gt_xyz, const float* m_xyz, const float* m_mask,
+                                const float* m_region, const long long* labels, const double* sums, const float* gw,
+                                const void* din_hi, const void* din_lo, const float* extents, void* out_hi, void* out_lo, int B,
+                                int HW, int with_2d, int mask_loss, int mask_out, void* stream_) {
     cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
-    GDRN_CUDA_OK(cudaMemsetAsync(sums, 0, 6 * sizeof(double), stream));
-    pixel_loss_fwd_kernel<<<px_grid((long)B * HW), 128, 0, stream>>>(logits, gt_xyz, m_visib, m_trunc, labels, sums, B, HW);
+    if (int rc = check_mask_head("head_bwd", mask_loss, mask_out)) return rc;
+    const bool sep = m_region != m_xyz;
+#define HB(MODE, MO, SEP) \
+    head_bwd_launch<MODE, MO, SEP>(logits, gt_xyz, m_xyz, m_mask, m_region, labels, sums, gw, din_hi, din_lo, extents, out_hi, out_lo, B, HW, with_2d, stream)
+    if (mask_loss == kMaskL1) {
+        if (sep) HB(kMaskL1, 1, true);
+        else HB(kMaskL1, 1, false);
+    } else if (mask_loss == kMaskBCE) {
+        if (sep) HB(kMaskBCE, 1, true);
+        else HB(kMaskBCE, 1, false);
+    } else {
+        if (sep) HB(kMaskCE, 2, true);
+        else HB(kMaskCE, 2, false);
+    }
+#undef HB
     GDRN_CUDA_OK(cudaGetLastError());
     count_launch();
     return 0;
@@ -714,18 +850,9 @@ extern "C" int gdrn_head_bwd(const float* logits, const float* gt_xyz, const flo
                              const long long* labels, const double* sums, const float* gw, const void* din_hi,
                              const void* din_lo, const float* extents, void* out_hi, void* out_lo, int B, int HW,
                              int with_2d, void* stream_) {
-    cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
-    if (with_2d)
-        head_bwd_kernel<true><<<px_grid((long)B * HW), 128, 0, stream>>>(logits, gt_xyz, m_visib, m_trunc, labels, sums, gw,
-                                                                        (const bf16*)din_hi, (const bf16*)din_lo, extents,
-                                                                        (bf16*)out_hi, (bf16*)out_lo, B, HW);
-    else
-        head_bwd_kernel<false><<<px_grid((long)B * HW), 128, 0, stream>>>(logits, gt_xyz, m_visib, m_trunc, labels, sums, gw,
-                                                                         (const bf16*)din_hi, (const bf16*)din_lo, extents,
-                                                                         (bf16*)out_hi, (bf16*)out_lo, B, HW);
-    GDRN_CUDA_OK(cudaGetLastError());
-    count_launch();
-    return 0;
+    // the same mask pointer for xyz and region: the kernel reads only sums[5], so six-slot buffers stay valid
+    return gdrn_head_bwd_ex(logits, gt_xyz, m_visib, m_trunc, m_visib, labels, sums, gw, din_hi, din_lo, extents, out_hi, out_lo, B,
+                            HW, with_2d, kMaskL1, 1, stream_);
 }
 
 extern "C" int gdrn_pose_loss(const float* pred, int ld_pred, const float* cams, const float* centers, const float* whs,
@@ -767,11 +894,20 @@ extern "C" int gdrn_pose_loss(const float* pred, int ld_pred, const float* cams,
     return 0;
 }
 
-extern "C" int gdrn_loss_finalize(const double* pix_sums, const double* pose_sums, const float* vis, float* losses,
-                                  float* vis_out, int B, int HW, int n_pts, void* stream_) {
-    cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
-    loss_finalize_kernel<<<1, 32, 0, stream>>>(pix_sums, pose_sums, vis, losses, vis_out, B, HW, n_pts);
+static int loss_finalize_launch(const double* pix_sums, const double* pose_sums, const float* vis, float* losses, float* vis_out,
+                                int B, int HW, int n_pts, int reg_slot, cudaStream_t stream) {
+    loss_finalize_kernel<<<1, 32, 0, stream>>>(pix_sums, pose_sums, vis, losses, vis_out, B, HW, n_pts, reg_slot);
     GDRN_CUDA_OK(cudaGetLastError());
     count_launch();
     return 0;
+}
+
+extern "C" int gdrn_loss_finalize_ex(const double* pix_sums, const double* pose_sums, const float* vis, float* losses,
+                                     float* vis_out, int B, int HW, int n_pts, void* stream_) {
+    return loss_finalize_launch(pix_sums, pose_sums, vis, losses, vis_out, B, HW, n_pts, 6, reinterpret_cast<cudaStream_t>(stream_));
+}
+
+extern "C" int gdrn_loss_finalize(const double* pix_sums, const double* pose_sums, const float* vis, float* losses,
+                                  float* vis_out, int B, int HW, int n_pts, void* stream_) {
+    return loss_finalize_launch(pix_sums, pose_sums, vis, losses, vis_out, B, HW, n_pts, 5, reinterpret_cast<cudaStream_t>(stream_));
 }

@@ -596,7 +596,7 @@ __global__ void __launch_bounds__(kGatherThreads) pnp_gather_kernel(const float*
     __shared__ float s_min[kGatherWarps], s_max[kGatherWarps];
     __shared__ int s_warp[kGatherWarps];
     __shared__ int s_base;
-    const float* m = mask + (long)b * HW;
+    const float* m = mask + (long)b * HW * (mask_mode == 3 ? 2 : 1);  // mode 3: two mask planes per ROI
     float mn = INFINITY, mx = -INFINITY;
     if (mask_mode == 1) {  // L1 mask head: per-ROI min-max normalisation (engine_utils.py:113-118)
         for (int i = tid; i < HW; i += kGatherThreads) {
@@ -633,6 +633,7 @@ __global__ void __launch_bounds__(kGatherThreads) pnp_gather_kernel(const float*
             float mv = m[i];
             if (mask_mode == 1) mv = __fdiv_rn(__fsub_rn(mv, mn), __fsub_rn(mx, mn));
             else if (mask_mode == 2) mv = 1.f / (1.f + expf(-mv));
+            else if (mask_mode == 3) mv = m[HW + i] > mv ? 1.f : 0.f;  // CE head: argmax over 2 channels, a tie is class 0
             X = __fmul_rn(__fsub_rn(xyz[((long)b * 3 + 0) * HW + i], 0.5f), ex);
             Y = __fmul_rn(__fsub_rn(xyz[((long)b * 3 + 1) * HW + i], 0.5f), ey);
             Z = __fmul_rn(__fsub_rn(xyz[((long)b * 3 + 2) * HW + i], 0.5f), ez);
@@ -1132,7 +1133,7 @@ extern "C" int gdrn_pnp_iterative(const float* mask, const float* xyz, const flo
     cudaStream_t stream = (cudaStream_t)stream_;
     if (!mask || !xyz || !coord2d || !extents || !im_wh || !K || !R_init || !t_init || !workspace || !out_pose || !out_info)
         return set_error(GDRN_ERR_ARG, "gdrn_pnp_iterative: null pointer");
-    if (B <= 0 || H <= 0 || W <= 0 || max_iters <= 0 || max_iters > 1000 || mask_mode < 0 || mask_mode > 2)
+    if (B <= 0 || H <= 0 || W <= 0 || max_iters <= 0 || max_iters > 1000 || mask_mode < 0 || mask_mode > 3)
         return set_error(GDRN_ERR_ARG, "gdrn_pnp_iterative: bad sizes (B=%d H=%d W=%d max_iters=%d mask_mode=%d)", B, H, W, max_iters,
                          mask_mode);
     const int HW = H * W;
@@ -1171,7 +1172,7 @@ extern "C" int gdrn_pnp_ransac(const float* mask, const float* xyz, const float*
     cudaStream_t stream = (cudaStream_t)stream_;
     if (!mask || !xyz || !coord2d || !extents || !im_wh || !K || !workspace || !out_pose || !out_info)
         return set_error(GDRN_ERR_ARG, "gdrn_pnp_ransac: null pointer");
-    if (B <= 0 || H <= 0 || W <= 0 || iters <= 0 || iters > 10000 || mask_mode < 0 || mask_mode > 2)
+    if (B <= 0 || H <= 0 || W <= 0 || iters <= 0 || iters > 10000 || mask_mode < 0 || mask_mode > 3)
         return set_error(GDRN_ERR_ARG, "gdrn_pnp_ransac: bad sizes (B=%d H=%d W=%d iters=%d mask_mode=%d)", B, H, W, iters, mask_mode);
     const int HW = H * W;
     if (workspace_bytes < gdrn_pnp_ransac_workspace_bytes(B, HW, iters))

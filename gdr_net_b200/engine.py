@@ -25,6 +25,7 @@ from .ops import PT, _stream
 from .patch_pnp import pnp_net_forward
 
 LOSS_NAMES = ["loss_coor_x", "loss_coor_y", "loss_coor_z", "loss_mask", "loss_region", "loss_PM_R", "loss_centroid", "loss_z"]
+MASK_LOSSES = {"L1": 0, "BCE": 1, "CE": 2}  # ROT_HEAD.MASK_LOSS_TYPE -> the mask_loss argument of the gdrn_*_ex loss kernels
 HEAD_CONVS = [(3, 4, False), (6, 7, False), (10, 11, True), (13, 14, False), (17, 18, True), (20, 21, False)]
 
 
@@ -115,6 +116,13 @@ class Engine:
         self.fold_eval = True  # inference by forward_eval_folded; False runs it through the unfused train-path kernels
         self.with_2d = int(model.pnp_net.features[0].in_channels == 69)  # 69 = xyz + coord2d + regions, 67 without coords
         assert model.pnp_net.features[0].in_channels in (67, 69), model.pnp_net.features[0].in_channels
+        # mask head (GDRN.py:339-400): MASK_LOSS_TYPE, the mask logits per pixel (1, or 2 for CE) and the GT mask of the xyz, mask
+        # and region losses (XYZ_LOSS_MASK_GT, MASK_LOSS_GT, REGION_LOSS_MASK_GT)
+        rh = model.cfg.MODEL.CDPN.ROT_HEAD
+        self.mask_loss = MASK_LOSSES[rh.MASK_LOSS_TYPE]
+        self.mask_out = model.rot_head_net.features[23].out_channels - 68  # mask | xyz | bg + 64 regions
+        assert self.mask_out == (2 if self.mask_loss == MASK_LOSSES["CE"] else 1), (self.mask_loss, self.mask_out)
+        self.mask_gt = (rh.XYZ_LOSS_MASK_GT, rh.MASK_LOSS_GT, rh.REGION_LOSS_MASK_GT)
         self.named_params = list(model.named_parameters())
         self.bn: Dict[str, _BN] = {}
         total = 0
@@ -331,15 +339,15 @@ class Engine:
 
     def _head_pnp(self, head_in: PT, aux: dict, pnp_saved: Optional[list] = None):
         """1x1 output conv -> glue -> Patch-PnP (GDRN.py:156-181, conv_pnp_net.py:111-157).  Returns the fp32 logits
-        [B*4096, 72], the Patch-PnP input planes, pred [B, 16] (cols 0..5 rot6d, 6..8 centroid dx, dy and z) and the inputs
+        [B*4096, 72] (68 + mask_out valid), the Patch-PnP input planes, pred [B, 16] (cols 0..5 rot6d, 6..8 centroid dx, dy and z) and the inputs
         of the three FC layers; pnp_saved receives the Patch-PnP conv activations (pnp_net_forward)."""
         m, B, dev = self.model, head_in.shape[0], self.dev
         logits = torch.empty(B * 4096, 72, device=dev)
-        ops.conv_fwd(head_in, self.wf["rot_head_net.features.23"], 69, 1, 1, 1, 0, out_f32=logits,
+        ops.conv_fwd(head_in, self.wf["rot_head_net.features.23"], 68 + self.mask_out, 1, 1, 1, 0, out_f32=logits,
                      bias=m.rot_head_net.features[23].bias, ldc=72, want_planes=False)
         pnp_in = PT((B, 64, 64, 128), self.planes, device=dev)
-        C.gdrn_head_glue_fwd(logits.data_ptr(), ops.ptr(aux.get("roi_coord_2d")), aux["roi_extents"].data_ptr(), pnp_in.hi_ptr,
-                             pnp_in.lo_ptr, B, 4096, self.with_2d, _stream())
+        C.gdrn_head_glue_fwd_ex(logits.data_ptr(), ops.ptr(aux.get("roi_coord_2d")), aux["roi_extents"].data_ptr(), pnp_in.hi_ptr,
+                                pnp_in.lo_ptr, B, 4096, self.with_2d, self.mask_out, _stream())
         pred = torch.zeros(B, 16, device=dev)
         fc_in = pnp_net_forward(pnp_in, m.pnp_net, self.wf, self.b_rt, pred, pnp_saved)
         return logits, pnp_in, pred, fc_in
@@ -357,7 +365,9 @@ class Engine:
         res = dict(rot=out_rot, trans=out_trans, pred=pred, logits=logits)
         if want_maps:
             maps = logits.view(B, 64, 64, 72).permute(0, 3, 1, 2)
-            res.update(mask=maps[:, 0:1], coor_x=maps[:, 1:2], coor_y=maps[:, 2:3], coor_z=maps[:, 3:4], region=maps[:, 4:69])
+            mo = self.mask_out
+            res.update(mask=maps[:, 0:mo], coor_x=maps[:, mo:mo + 1], coor_y=maps[:, mo + 1:mo + 2], coor_z=maps[:, mo + 2:mo + 3],
+                       region=maps[:, mo + 3:mo + 68])
         return res
 
     def _prepare_weights_calls(self, need_dgrad: bool):
@@ -426,12 +436,12 @@ class Engine:
 
     # ------------------------------------------------------------------------------------------ forward
     def run(self, x, *, roi_coord_2d, roi_cams, roi_centers, roi_whs, roi_extents, resize_ratios, gt_xyz=None,
-            gt_mask_trunc=None, gt_mask_visib=None, gt_region=None, gt_ego_rot=None, gt_points=None, sym_infos=None,
-            gt_trans=None, gt_trans_ratio=None, do_loss=False, train_bn=False, want_maps=False):
+            gt_mask_trunc=None, gt_mask_visib=None, gt_mask_obj=None, gt_region=None, gt_ego_rot=None, gt_points=None,
+            sym_infos=None, gt_trans=None, gt_trans_ratio=None, do_loss=False, train_bn=False, want_maps=False):
         aux = dict(roi_coord_2d=roi_coord_2d, roi_cams=roi_cams, roi_centers=roi_centers, roi_whs=roi_whs,
                    roi_extents=roi_extents, resize_ratios=resize_ratios, gt_xyz=gt_xyz, gt_mask_trunc=gt_mask_trunc,
-                   gt_mask_visib=gt_mask_visib, gt_region=gt_region, gt_ego_rot=gt_ego_rot, gt_points=gt_points,
-                   sym_infos=sym_infos, gt_trans=gt_trans, gt_trans_ratio=gt_trans_ratio)
+                   gt_mask_visib=gt_mask_visib, gt_mask_obj=gt_mask_obj, gt_region=gt_region, gt_ego_rot=gt_ego_rot,
+                   gt_points=gt_points, sym_infos=sym_infos, gt_trans=gt_trans, gt_trans_ratio=gt_trans_ratio)
         B = x.shape[0]
         for k_, v in aux.items():
             if isinstance(v, torch.Tensor):
@@ -443,7 +453,7 @@ class Engine:
             aux["roi_cams"] = aux["roi_cams"].unsqueeze(0).expand(B, 3, 3).contiguous()
         want = dict(roi_coord_2d=(B, 2, 64, 64), roi_cams=(B, 3, 3), roi_centers=(B, 2), roi_whs=(B, 2), roi_extents=(B, 3),
                     resize_ratios=(B,), gt_xyz=(B, 3, 64, 64), gt_mask_trunc=(B, 64, 64), gt_mask_visib=(B, 64, 64),
-                    gt_region=(B, 64, 64), gt_ego_rot=(B, 3, 3), gt_trans=(B, 3), gt_trans_ratio=(B, 3))
+                    gt_mask_obj=(B, 64, 64), gt_region=(B, 64, 64), gt_ego_rot=(B, 3, 3), gt_trans=(B, 3), gt_trans_ratio=(B, 3))
         for k_, shp in want.items():
             v = aux.get(k_)
             if isinstance(v, torch.Tensor):
@@ -537,9 +547,10 @@ class Engine:
         logits, pnp_in, pred, (flat, h1, h2) = self._head_pnp(head_in, aux, pnp_saved)
 
         # ---- a5/a6 pose decode + a7..a10 losses
-        pix_sums = torch.empty(6, dtype=torch.float64, device=dev)
-        C.gdrn_pixel_loss_fwd(logits.data_ptr(), aux["gt_xyz"].data_ptr(), aux["gt_mask_visib"].data_ptr(),
-                              aux["gt_mask_trunc"].data_ptr(), aux["gt_region"].data_ptr(), pix_sums.data_ptr(), B, 4096, _stream())
+        pix_sums = torch.empty(7, dtype=torch.float64, device=dev)
+        m_xyz, m_mask, m_region = self._loss_masks(aux)
+        C.gdrn_pixel_loss_fwd_ex(logits.data_ptr(), aux["gt_xyz"].data_ptr(), m_xyz, m_mask, m_region, aux["gt_region"].data_ptr(),
+                                 pix_sums.data_ptr(), B, 4096, self.mask_loss, self.mask_out, _stream())
         S.update(logits=logits, pnp_in=pnp_in, pnp=pnp_saved, flat=flat, h1=h1, h2=h2, pred=pred, head_in=head_in,
                  pix_sums=pix_sums, aux=aux)
         self.saved = S
@@ -549,10 +560,21 @@ class Engine:
         losses = torch.empty(8, device=dev)
         vis2 = torch.empty(2, device=dev)
         n_pts = aux["gt_points"].shape[1]
-        C.gdrn_loss_finalize(pix_sums.data_ptr(), S["pose_sums"].data_ptr(), S["vis_ps"].data_ptr(), losses.data_ptr(),
-                             vis2.data_ptr(), B, 4096, n_pts, _stream())
+        C.gdrn_loss_finalize_ex(pix_sums.data_ptr(), S["pose_sums"].data_ptr(), S["vis_ps"].data_ptr(), losses.data_ptr(),
+                                vis2.data_ptr(), B, 4096, n_pts, _stream())
         vis = torch.cat([vis2, S["out_trans"][0], pred[0, 6:9], aux["gt_trans"][0], aux["gt_trans_ratio"][0]])
         return dict(rot=S["out_rot"], trans=S["out_trans"], pred=pred, losses=losses, vis=vis, logits=logits)
+
+    def _loss_masks(self, aux) -> tuple:
+        """Device pointers of the GT masks that weight the xyz loss, are the mask loss's target and weight the region loss
+        (gt_masks[XYZ_LOSS_MASK_GT], [MASK_LOSS_GT], [REGION_LOSS_MASK_GT], GDRN.py:339-395); the same mask gives the same pointer."""
+        out = []
+        for sel in self.mask_gt:
+            m = aux.get("gt_mask_" + sel)
+            if not isinstance(m, torch.Tensor):
+                raise ValueError(f"the loss configuration selects gt_mask_{sel}, which was not given")
+            out.append(m.data_ptr())
+        return tuple(out)
 
     def _pose(self, S, gw):
         aux, B, dev = S["aux"], S["B"], self.dev
@@ -674,20 +696,21 @@ class Engine:
 
         # ---- glue + per-pixel losses backward (one fused pass over the logits)
         dlog = PT((B * 4096, 128), bp, device=dev)
-        C.gdrn_head_bwd(S["logits"].data_ptr(), aux["gt_xyz"].data_ptr(), aux["gt_mask_visib"].data_ptr(),
-                        aux["gt_mask_trunc"].data_ptr(), aux["gt_region"].data_ptr(), S["pix_sums"].data_ptr(), gw.data_ptr(),
-                        d_pnp_in.hi_ptr, d_pnp_in.lo_ptr, aux["roi_extents"].data_ptr(), dlog.hi_ptr, dlog.lo_ptr, B, 4096,
-                        self.with_2d, _stream())
+        m_xyz, m_mask, m_region = self._loss_masks(aux)
+        C.gdrn_head_bwd_ex(S["logits"].data_ptr(), aux["gt_xyz"].data_ptr(), m_xyz, m_mask, m_region, aux["gt_region"].data_ptr(),
+                           S["pix_sums"].data_ptr(), gw.data_ptr(), d_pnp_in.hi_ptr, d_pnp_in.lo_ptr, aux["roi_extents"].data_ptr(),
+                           dlog.hi_ptr, dlog.lo_ptr, B, 4096, self.with_2d, self.mask_loss, self.mask_out, _stream())
         hf = m.rot_head_net.features
         head_in = h(S["head_in"])
+        n_out = 68 + self.mask_out  # rows of the 1x1 output conv
         def head_out_wgrad():
             buf, ks, kss = ops.gemm_wgrad(dlog, head_in.view(B * 4096, 256), self.ws)
-            ops.unpack_wgrad(buf, self.grads["rot_head_net.features.23.weight"], 69, 256, 1, 1, 256, ks, kss, 256, 1, 0, 0)
+            ops.unpack_wgrad(buf, self.grads["rot_head_net.features.23.weight"], n_out, 256, 1, 1, 256, ks, kss, 256, 1, 0, 0)
 
         self._on_side(head_out_wgrad, keep=(dlog,))
         tmp128 = torch.empty(128, device=dev)
         C.gdrn_colsum(dlog.hi_ptr, dlog.lo_ptr, tmp128.data_ptr(), B * 4096, 128, _stream())
-        self.grads["rot_head_net.features.23.bias"].copy_(tmp128[:69])
+        self.grads["rot_head_net.features.23.bias"].copy_(tmp128[:n_out])
         g = ops.gemm_fwd(dlog, self.wd["rot_head_net.features.23"], 256).view(B, 64, 64, 256)
 
         # ---- head convs (cdpn_rot_head_region.py:95-125)

@@ -18,13 +18,22 @@ import torch
 
 from .capi import C
 
-_MASK_MODES = {"none": 0, "L1": 1, "BCE": 2}
+_MASK_MODES = {"none": 0, "L1": 1, "BCE": 2, "CE": 3}
+
+
+def _mask_planes(mask: torch.Tensor, mask_loss_type: str, B: int, h: int, w: int) -> torch.Tensor:
+    """The mask head output as the kernels read it: [B, h*w], or [B, 2*h*w] (two planes per ROI) for the CE head."""
+    n = 2 if mask_loss_type == "CE" else 1
+    if mask.numel() != B * n * h * w:
+        raise ValueError(f"mask: expected {n} channel(s) of {h}x{w} per ROI for mask_loss_type {mask_loss_type!r}, got {tuple(mask.shape)}")
+    return mask.reshape(B, n * h * w)
 
 
 def pnp_ransac(mask: torch.Tensor, xyz: torch.Tensor, coord_2d: torch.Tensor, extents: torch.Tensor, im_wh, cams: torch.Tensor,
                mask_loss_type: str = "L1", mask_thr: float = 0.5, reproj_err: float = 3.0, iters: int = 100,
                confidence: float = 0.99, return_inliers: bool = False) -> dict:
-    """mask [B,1,h,w] raw head output (normalised here like `get_out_mask` for `mask_loss_type` "L1" / "BCE"; "none": used as is),
+    """mask [B,1,h,w] raw head output (normalised here like `get_out_mask` for `mask_loss_type` "L1" / "BCE"; "none": used as is)
+    or [B,2,h,w] for the CE mask head (`mask_loss_type` "CE": argmax over the two channels, a tie selecting class 0),
     xyz [B,3,h,w] in [0,1] (`get_out_coor` of the regression head = cat(coor_x, coor_y, coor_z)), coord_2d [B,2,h,w] in [0,1],
     extents [B,3], im_wh [B,2] or (W, H), cams [B,3,3] or [3,3].
     Returns dict(pose [B,3,4], num_points [B], num_inliers [B], iterations [B], ok [B] (bool)[, inliers [B,h*w] uint8 flags over
@@ -33,11 +42,11 @@ def pnp_ransac(mask: torch.Tensor, xyz: torch.Tensor, coord_2d: torch.Tensor, ex
     if not mask.is_cuda:
         raise RuntimeError("gdr_net_b200.pnp_ransac runs on CUDA only; there is no CPU fallback")
     if mask_loss_type not in _MASK_MODES:
-        raise NotImplementedError(f"unknown mask loss type: {mask_loss_type}")  # "CE" masks are not produced by the shipped configs
+        raise NotImplementedError(f"unknown mask loss type: {mask_loss_type}")
     dev = mask.device
     B, _, h, w = xyz.shape
     f = lambda t: t.detach().to(dev).float().contiguous()  # noqa: E731
-    mask, xyz, coord_2d, extents = f(mask).reshape(B, h * w), f(xyz), f(coord_2d), f(extents).reshape(B, 3)
+    mask, xyz, coord_2d, extents = _mask_planes(f(mask), mask_loss_type, B, h, w), f(xyz), f(coord_2d), f(extents).reshape(B, 3)
     if coord_2d.shape != (B, 2, h, w):
         raise ValueError(f"pnp_ransac: coord_2d {tuple(coord_2d.shape)} does not match xyz {tuple(xyz.shape)}")
     if not torch.is_tensor(im_wh):
@@ -98,7 +107,7 @@ def pnp_iterative(mask: torch.Tensor, xyz: torch.Tensor, coord_2d: torch.Tensor,
     dev = mask.device
     B, _, h, w = xyz.shape
     f = lambda t: t.detach().to(dev).float().contiguous()  # noqa: E731
-    mask, xyz, coord_2d, extents = f(mask).reshape(B, h * w), f(xyz), f(coord_2d), f(extents).reshape(B, 3)
+    mask, xyz, coord_2d, extents = _mask_planes(f(mask), mask_loss_type, B, h, w), f(xyz), f(coord_2d), f(extents).reshape(B, 3)
     if coord_2d.shape != (B, 2, h, w):
         raise ValueError(f"pnp_iterative: coord_2d {tuple(coord_2d.shape)} does not match xyz {tuple(xyz.shape)}")
     R_init, t_init = f(R_init).reshape(B, 3, 3), f(t_init).reshape(B, 3)

@@ -151,6 +151,23 @@ int gdrn_pixel_loss_fwd(const float* logits, const float* gt_xyz, const float* m
 int gdrn_head_bwd(const float* logits, const float* gt_xyz, const float* m_visib, const float* m_trunc,
                   const long long* labels, const double* sums, const float* gw, const void* din_hi, const void* din_lo,
                   const float* extents, void* out_hi, void* out_lo, int B, int HW, int with_2d, void* stream);
+/* The same with the mask head and the GT masks selectable (ROT_HEAD.MASK_LOSS_TYPE, XYZ_LOSS_MASK_GT, MASK_LOSS_GT,
+ * REGION_LOSS_MASK_GT; GDRN.py:339-400).  mask_loss 0 = L1, 1 = BCE (BCEWithLogits mean), 2 = CE (2-class CrossEntropy mean,
+ * label = (int) target); mask_out = mask logits per pixel, 1 for L1 / BCE and 2 for CE.  Logit row: mask [0, mask_out) | xyz |
+ * bg | 64 regions, 68 + mask_out valid of 72.  m_xyz weights and normalises the xyz L1, m_mask is the mask-loss target,
+ * m_region weights and normalises the region CE; they may be the same pointer.  sums double[7]: |dx|, |dy|, |dz|, mask loss,
+ * region CE, sum(m_xyz), sum(m_region).  head_bwd_ex zeroes gradient columns 68 + mask_out .. 127.  The original four entry
+ * points above are these with (mask_loss 0, mask_out 1, m_xyz = m_region = m_visib, m_mask = m_trunc) and six sums, slot 5
+ * serving both normalisers. */
+int gdrn_head_glue_fwd_ex(const float* logits, const float* coord2d, const float* extents, void* out_hi, void* out_lo, int B,
+                          int HW, int with_2d, int mask_out, void* stream);
+int gdrn_pixel_loss_fwd_ex(const float* logits, const float* gt_xyz, const float* m_xyz, const float* m_mask,
+                           const float* m_region, const long long* labels, double* sums, int B, int HW, int mask_loss,
+                           int mask_out, void* stream);
+int gdrn_head_bwd_ex(const float* logits, const float* gt_xyz, const float* m_xyz, const float* m_mask, const float* m_region,
+                     const long long* labels, const double* sums, const float* gw, const void* din_hi, const void* din_lo,
+                     const float* extents, void* out_hi, void* out_lo, int B, int HW, int with_2d, int mask_loss, int mask_out,
+                     void* stream);
 
 /* ---- rot6d -> R, SITE translation, allo -> ego, PM loss (+ closest symmetric GT), centroid / z losses, re/te
  * (rot_reps.py:34-49, pose_from_pred_centroid_z.py:144-227, utils.py:208-236, pm_loss.py:82-114,
@@ -164,6 +181,9 @@ int gdrn_pose_loss(const float* pred, int ld_pred, const float* cams, const floa
                    int do_loss, float eps, void* stream);
 int gdrn_loss_finalize(const double* pix_sums, const double* pose_sums, const float* vis, float* losses, float* vis_out,
                        int B, int HW, int n_pts, void* stream);
+/* pix_sums of gdrn_pixel_loss_fwd_ex (7 slots): the region loss is normalised by slot 6 */
+int gdrn_loss_finalize_ex(const double* pix_sums, const double* pose_sums, const float* vis, float* losses, float* vis_out,
+                          int B, int HW, int n_pts, void* stream);
 
 /* ---- per-instance crop / target generation of the data loader on the device (core/gdrn_modeling/data_loader.py:487-560,
  * core/utils/data_utils.py:80-137 crop_resize_by_warp_affine, :213-219 xyz_to_region), cv2.warpAffine's fixed-point sampling
@@ -187,7 +207,8 @@ int gdrn_pose_errors(const float* R_est, const float* t_est, const float* R_gt, 
 /* ---- test-time RANSAC-PnP of the evaluator on the device (core/gdrn_modeling/gdrn_evaluator.py:316-436 `process_pnp_ransac`:
  * `get_img_model_points_with_coords2d` :89-126 + lib/pysixd/misc.py:145-194 `pnp_v2` = cv2.solvePnPRansac(EPNP, reprojErr 3, 100
  * iterations) per instance on the host).  mask [B][H*W] (mask_mode 0: used as is, 1: per-ROI min-max normalised like
- * engine_utils.py:113-118 for the L1 mask head, 2: sigmoid), xyz [B][3][H*W] in [0,1], coord2d [B][2][H*W] in [0,1],
+ * engine_utils.py:113-118 for the L1 mask head, 2: sigmoid) or [B][2][H*W] (mask_mode 3, the CE mask head: argmax over the two
+ * channels, a tie giving 0, engine_utils.py:123-124), compared with mask_thr; xyz [B][3][H*W] in [0,1], coord2d [B][2][H*W] in [0,1],
  * extents [B][3], im_wh [B][2] = (im_W, im_H), K [B][3][3].  out_pose [B][3][4] = [R | t]; out_info [B][4] = (selected points,
  * inliers, RANSAC iterations run, ok); out_inliers (optional) [B][H*W] flags indexed like cv2's inlier list (position in the
  * row-major list of selected points).  Follows OpenCV's algorithm (RNG-driven 5-point subsets, EPnP minimal + final solver,
