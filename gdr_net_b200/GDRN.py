@@ -18,7 +18,7 @@ from typing import Optional
 import torch
 import torch.nn as nn
 
-from .engine import Engine, LOSS_NAMES
+from .engine import Engine, LOSS_NAMES, pose_loss_switches  # noqa: F401  (LOSS_NAMES: the default list, re-exported)
 
 logger = logging.getLogger(__name__)
 
@@ -202,15 +202,17 @@ def _check_supported(cfg):
         if getattr(r, key) not in ("trunc", "visib", "obj"):
             problems.append(f"ROT_HEAD.{key} = {getattr(r, key)!r} (trunc, visib or obj)")
     if not p.REGION_ATTENTION or p.MASK_ATTENTION != "none" or p.R_ONLY:
-        problems.append("Patch-PnP input other than xyz (+ 2D coords) + region attention")
+        problems.append("Patch-PnP input other than xyz (+ 2D coords) + region attention (PNP_NET.REGION_ATTENTION, MASK_ATTENTION, R_ONLY)")
     if p.ROT_TYPE != "allo_rot6d" or p.TRANS_TYPE != "centroid_z" or p.Z_TYPE != "REL":
-        problems.append("pose parametrisation other than allo_rot6d + centroid_z(REL)")
-    if not (p.PM_R_ONLY and p.PM_NORM_BY_EXTENT) or p.PM_LOSS_TYPE != "L1" or p.PM_LW <= 0:
-        problems.append("PM loss other than r_only L1 norm_by_extent")
-    if p.ROT_LW > 0 or p.TRANS_LW > 0 or p.get("BIND_LW", 0.0) > 0 or p.CENTROID_LOSS_TYPE != "L1" or p.Z_LOSS_TYPE != "L1":
-        problems.append("rot/trans/bind losses or non-L1 centroid/z losses")
+        problems.append(f"pose parametrisation other than allo_rot6d + centroid_z(REL) (PNP_NET.ROT_TYPE = {p.ROT_TYPE!r}, "
+                        f"TRANS_TYPE = {p.TRANS_TYPE!r}, Z_TYPE = {p.Z_TYPE!r})")
+    # the PNP_NET loss switches (PM_*, ROT_*, CENTROID_*, Z_*, TRANS_*, BIND_*): engine.pose_loss_switches names a bad one
+    try:
+        pose_loss_switches(p)
+    except ValueError as e:
+        problems.append(str(e))
     if c.TRANS_HEAD.ENABLED or c.USE_MTL or c.BACKBONE.FREEZE or r.FREEZE or p.FREEZE:
-        problems.append("trans head / MTL weighting / frozen sub-nets")
+        problems.append("trans head / MTL weighting / frozen sub-nets (TRANS_HEAD.ENABLED, USE_MTL, FREEZE)")
     if problems:
         raise NotImplementedError("gdr_net_b200 implements the a6_cPnP hot path only; unsupported: " + "; ".join(problems))
 
@@ -284,10 +286,16 @@ class GDRN(nn.Module):
         assert (gt_xyz is not None) and (gt_trans is not None) and (gt_trans_ratio is not None) and (gt_region is not None)
         r_cfg = cfg.MODEL.CDPN.ROT_HEAD
         lw = dict(loss_coor_x=r_cfg.XYZ_LW, loss_coor_y=r_cfg.XYZ_LW, loss_coor_z=r_cfg.XYZ_LW, loss_mask=r_cfg.MASK_LW,
-                  loss_region=r_cfg.REGION_LW, loss_PM_R=pnp_cfg.PM_LW, loss_centroid=pnp_cfg.CENTROID_LW, loss_z=pnp_cfg.Z_LW)
-        losses = res["losses"]  # [8] tensor attached to the autograd graph through _GDRNFunction
+                  loss_region=r_cfg.REGION_LW, loss_rot=pnp_cfg.ROT_LW, loss_centroid=pnp_cfg.CENTROID_LW, loss_z=pnp_cfg.Z_LW,
+                  loss_trans_xy=pnp_cfg.TRANS_LW, loss_trans_z=pnp_cfg.TRANS_LW, loss_trans_LPnP=pnp_cfg.TRANS_LW,
+                  loss_bind=pnp_cfg.get("BIND_LW", 0.0))
+        for name in ("loss_PM_R", "loss_PM_RT", "loss_PM_T", "loss_PM_xy", "loss_PM_z"):
+            lw[name] = pnp_cfg.PM_LW
+        for name in ("loss_PM_T_noP", "loss_PM_xy_noP", "loss_PM_z_noP"):  # pm_loss.py:146-164: neither PM_LW nor 3
+            lw[name] = 1.0
+        losses = res["losses"]  # [len(engine.loss_names)] tensor attached to the autograd graph through _GDRNFunction
         loss_dict = {}
-        for i, name in enumerate(LOSS_NAMES):
+        for i, name in enumerate(self.engine.loss_names):
             if name in ("loss_centroid", "loss_z") and lw[name] <= 0:
                 continue
             loss_dict[name] = losses[i] * lw[name]

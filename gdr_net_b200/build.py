@@ -46,6 +46,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
     os.makedirs(BUILD, exist_ok=True)
     os.makedirs(LIBDIR, exist_ok=True)
     headers = [os.path.join(CSRC, f) for f in sorted(os.listdir(CSRC)) if f.endswith((".h", ".cuh"))]
+    headers.append(os.path.join(os.path.dirname(HERE), "include", "gdrn_b200.h"))  # losses.cu includes the public header
     jobs = []
     objs = []
     for src in _sources():

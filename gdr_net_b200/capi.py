@@ -14,6 +14,18 @@ _SCALARS = {"int": ctypes.c_int, "long": ctypes.c_long, "float": ctypes.c_float,
             "long long": ctypes.c_longlong}
 
 
+class PoseSwitches(ctypes.Structure):
+    """gdrn_pose_switches of include/gdrn_b200.h (passed by value)."""
+
+    _fields_ = [("pm_mode", ctypes.c_int), ("pm_type", ctypes.c_int), ("pm_beta", ctypes.c_float),
+                ("pm_norm_extent", ctypes.c_int), ("rot_type", ctypes.c_int), ("centroid_type", ctypes.c_int),
+                ("z_type", ctypes.c_int), ("trans_type", ctypes.c_int), ("trans_disentangle", ctypes.c_int),
+                ("bind_type", ctypes.c_int)]
+
+
+_SCALARS["gdrn_pose_switches"] = PoseSwitches
+
+
 def parse_header(path: str = HEADER) -> dict:
     """name -> (restype, [argtypes]) for every `gdrn_*` prototype in the public header."""
     txt = open(path).read()

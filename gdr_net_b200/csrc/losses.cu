@@ -11,6 +11,7 @@
 //                   model_utils.py:40-52 (mean re / te logging) -- forward + analytic/forward-mode backward.
 #include <math.h>
 
+#include "../../include/gdrn_b200.h"
 #include "gdrn_internal.h"
 #include "ptx.cuh"
 
@@ -430,6 +431,98 @@ __device__ __forceinline__ void dnormalize3(Dual (&v)[3]) {
     for (int i = 0; i < 3; ++i) v[i] = v[i] / n;
 }
 
+// ------------------------------------------------------------------------------------------------
+// PNP_NET pose-loss switches (gdrn_pose_switches).  Every loss is a per-crop partial in one of GDRN_POSE_SLOTS slots; the
+// active slots, ascending, are the reference's loss_dict order (PyPMLoss entries, rot, centroid, z, trans, bind).
+// ------------------------------------------------------------------------------------------------
+enum PoseLoss { kLossL1 = 0, kLossSmoothL1 = 1, kLossMSE = 2, kLossL2 = 3 };
+enum PmMode { kPmOff = -1, kPmR = 0, kPmRT = 1, kPmDisT = 2, kPmDisZ = 3, kPmDisTNoP = 4, kPmDisZNoP = 5 };
+enum PoseSlot { kSlotPmR = 0, kSlotPmT = 1, kSlotPmZ = 2, kSlotNoP = 3, kSlotNoPZ = 4, kSlotRot = 5, kSlotCentroid = 6, kSlotZ = 7,
+                kSlotTrans = 8, kSlotTransZ = 9, kSlotBind = 10 };
+
+__host__ __device__ inline unsigned pose_slot_mask(const gdrn_pose_switches& sw) {
+    unsigned m = (1u << kSlotCentroid) | (1u << kSlotZ);
+    switch (sw.pm_mode) {
+        case kPmR: case kPmRT: m |= 1u << kSlotPmR; break;
+        case kPmDisT: m |= (1u << kSlotPmR) | (1u << kSlotPmT); break;
+        case kPmDisZ: m |= (1u << kSlotPmR) | (1u << kSlotPmT) | (1u << kSlotPmZ); break;
+        case kPmDisTNoP: m |= (1u << kSlotPmR) | (1u << kSlotNoP); break;
+        case kPmDisZNoP: m |= (1u << kSlotPmR) | (1u << kSlotNoP) | (1u << kSlotNoPZ); break;
+        default: break;
+    }
+    if (sw.rot_type >= 0) m |= 1u << kSlotRot;
+    if (sw.trans_type >= 0) m |= sw.trans_disentangle ? (1u << kSlotTrans) | (1u << kSlotTransZ) : (1u << kSlotTrans);
+    if (sw.bind_type >= 0) m |= 1u << kSlotBind;
+    return m;
+}
+
+// loss_s = fac * sum_b part[b][s] / den.  Elementwise kinds take the mean over every element (the PM entries carry the
+// reference's factor 3 over B n 3 elements: 1 / (B n)); L2 is the mean over B of per-crop norms (3 / B for the PM entries).
+__host__ __device__ inline double pose_slot_den(const gdrn_pose_switches& sw, int s, int B, int n_pts, double* fac) {
+    *fac = 1.0;
+    const bool l2_pm = sw.pm_type == kLossL2;
+    switch (s) {
+        case kSlotPmR: case kSlotPmT: case kSlotPmZ:
+            if (l2_pm) {
+                *fac = 3.0;
+                return (double)B;
+            }
+            return (double)B * n_pts;
+        case kSlotNoP: return l2_pm ? (double)B : (sw.pm_mode == kPmDisTNoP ? 3.0 : 2.0) * B;
+        case kSlotRot: return sw.rot_type == 1 ? 9.0 * B : (double)B;
+        case kSlotCentroid: return sw.centroid_type == kLossL2 ? (double)B : 2.0 * B;
+        case kSlotTrans:
+            return sw.trans_type == kLossL2 ? (double)B : (sw.trans_disentangle ? 2.0 : 3.0) * B;
+        case kSlotBind: return sw.bind_type == kLossL2 ? (double)B : 3.0 * B;
+        default: return (double)B;  // z_noP, z, trans z: one element per crop
+    }
+}
+
+// one residual e: value v and dv/de of L1 | Smooth-L1 (torch / fvcore: 0.5 e^2 / beta below beta, |e| - 0.5 beta above, L1 for
+// beta < 1e-5) | MSE; for L2 v = e^2 and g = e (the norm and its 1 / ||e|| are applied per crop)
+__device__ __forceinline__ void pose_elem(int kind, float e, float beta, float& v, float& g) {
+    const float a = fabsf(e);
+    const float sg = e > 0.f ? 1.f : (e < 0.f ? -1.f : 0.f);
+    if (kind == kLossSmoothL1 && beta >= 1e-5f) {
+        if (a < beta) {
+            v = __fmul_rn(__fmul_rn(0.5f, a), a) / beta;
+            g = e / beta;
+        } else {
+            v = a - __fmul_rn(0.5f, beta);
+            g = sg;
+        }
+    } else if (kind == kLossMSE) {
+        v = __fmul_rn(e, e);
+        g = 2.f * e;
+    } else if (kind == kLossL2) {
+        v = __fmul_rn(e, e);
+        g = e;
+    } else {
+        v = a;
+        g = sg;
+    }
+}
+
+// a group of n residuals of one loss entry of one crop: returns the crop's partial, d = coef * d(partial)/de.  L2: the norm
+// sqrt(sum e^2) with d = coef e / ||e||, and d = 0 at ||e|| = 0 like torch.norm's gradient.
+__device__ __forceinline__ float pose_group(int kind, float beta, const float* e, int n, float coef, float* d) {
+    float s = 0.f;
+    if (kind == kLossL2) {
+        for (int i = 0; i < n; ++i) s += __fmul_rn(e[i], e[i]);
+        const float nrm = sqrtf(s);
+        const float c = nrm > 0.f ? coef / nrm : 0.f;
+        for (int i = 0; i < n; ++i) d[i] = c * e[i];
+        return nrm;
+    }
+    for (int i = 0; i < n; ++i) {
+        float v, g;
+        pose_elem(kind, e[i], beta, v, g);
+        s += v;
+        d[i] = coef * g;
+    }
+    return s;
+}
+
 struct PoseParams {
     const float* rot6d;   // [B][ld_pred] cols 0..5 (fc output fp32)
     const float* pred_t;  // [B][ld_pred] (pointer already offset to col 6)
@@ -455,13 +548,219 @@ struct PoseParams {
     int B, n_pts, do_loss;
     float eps;  // 1e-4 in the differentiable train decode (utils.py:208-236); 0 = exact normalisation of the test-time
                 // decode (pose_from_pred_centroid_z.py:52-141 -> utils.py:39-94 axangle2mat)
+    // EX only (gdrn_pose_loss_ex): the switches, per-crop partials [B][GDRN_POSE_SLOTS] instead of `sums`, and gw = the upstream
+    // gradients of the active slots in slot order
+    gdrn_pose_switches sw;
+    float* part;
 };
 
+// The losses of gdrn_pose_loss_ex after the decode and the symmetric search (sRgt: the PM target, sRg0: the original R_gt that
+// loss_rot and loss_bind use).  The per-point pass accumulates the three point-matching terms, dL/dR (G, as in the shipped
+// kernel) and dL/dT (GT); L2 needs no second pass because its gradient is sum(e p^T) / ||e|| per crop.  Thread 0 then adds the
+// per-crop losses on (R, T, pred_t) and contracts everything with the forward-mode Jacobians sJ (dR) and sJT (dT).
+__device__ __forceinline__ void pose_loss_ex_tail(const PoseParams& p, const float* sR, const float* sRgt, const float* sRg0,
+                                                  const float* sT, float (*sJ)[9], float (*sJT)[9], float* sG, float* sGT,
+                                                  float* sAcc, float (*red)[4]) {
+    const int b = blockIdx.x;
+    const gdrn_pose_switches& sw = p.sw;
+    const int mode = sw.pm_mode, kind = sw.pm_type;
+    const float beta = sw.pm_beta;
+    const float* Tgp = p.gt_trans + b * 3;
+    const float Tp[3] = {sT[0], sT[1], sT[2]}, Tg[3] = {Tgp[0], Tgp[1], Tgp[2]};
+    // weights * points (pm_loss.py:102-107): 1 / max extent, or exactly 1
+    const float w = sw.pm_norm_extent ? 1.f / fmaxf(fmaxf(p.extents[b * 3], p.extents[b * 3 + 1]), p.extents[b * 3 + 2]) : 1.f;
+    float acc[3] = {0.f, 0.f, 0.f}, G[9], GT[3] = {0.f, 0.f, 0.f};
+#pragma unroll
+    for (int i = 0; i < 9; ++i) G[i] = 0.f;
+    if (mode != kPmOff) {
+        const float* pts = p.points + (long)b * p.n_pts * 3;
+        for (int n = threadIdx.x; n < p.n_pts; n += blockDim.x) {
+            const float px = pts[n * 3], py = pts[n * 3 + 1], pz = pts[n * 3 + 2];
+#pragma unroll
+            for (int i = 0; i < 3; ++i) {
+                const float est = sR[i * 3] * px + sR[i * 3 + 1] * py + sR[i * 3 + 2] * pz;
+                const float tgt = sRgt[i * 3] * px + sRgt[i * 3 + 1] * py + sRgt[i * 3 + 2] * pz;
+                // rotation term: R p [+ t | + t_gt] against R_gt p [+ t_gt], each side weighted before the subtraction
+                float e;
+                if (mode == kPmRT) e = masked_diff(est + Tp[i], tgt + Tg[i], w);
+                else if (mode == kPmDisT || mode == kPmDisZ) e = masked_diff(est + Tg[i], tgt + Tg[i], w);
+                else e = masked_diff(est, tgt, w);
+                float v, g;
+                pose_elem(kind, e, beta, v, g);
+                acc[0] += v;
+                const float sg = g * w;
+                G[i * 3] += sg * px;
+                G[i * 3 + 1] += sg * py;
+                G[i * 3 + 2] += sg * pz;
+                if (mode == kPmRT) GT[i] += sg;
+                // translation terms with points: R_gt p + t (DISENTANGLE_T), or with t_gt's z (xy) / x, y (z) for DISENTANGLE_Z,
+                // whose other components are exactly 0 and are skipped
+                if (mode == kPmDisT || mode == kPmDisZ) {
+                    const float e1 = masked_diff(tgt + Tp[i], tgt + Tg[i], w);
+                    pose_elem(kind, e1, beta, v, g);
+                    acc[(mode == kPmDisZ && i == 2) ? 2 : 1] += v;
+                    GT[i] += g * w;
+                }
+            }
+        }
+    }
+    float vals[15];
+#pragma unroll
+    for (int j = 0; j < 3; ++j) vals[j] = acc[j];
+#pragma unroll
+    for (int j = 0; j < 9; ++j) vals[3 + j] = G[j];
+#pragma unroll
+    for (int j = 0; j < 3; ++j) vals[12 + j] = GT[j];
+#pragma unroll
+    for (int j = 0; j < 15; ++j) {
+        float v = vals[j];
+        for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+        if ((threadIdx.x & 31) == 0) red[j][threadIdx.x >> 5] = v;
+    }
+    __syncthreads();
+    if (threadIdx.x < 15) {
+        const float v = red[threadIdx.x][0] + red[threadIdx.x][1] + red[threadIdx.x][2] + red[threadIdx.x][3];
+        if (threadIdx.x < 3) sAcc[threadIdx.x] = v;
+        else if (threadIdx.x < 12) sG[threadIdx.x - 3] = v;
+        else sGT[threadIdx.x - 12] = v;
+    }
+    __syncthreads();
+    if (threadIdx.x != 0) return;
+
+    const unsigned mask = pose_slot_mask(sw);
+    auto coef = [&](int s) {  // upstream gradient * fac / den of slot s
+        double fac;
+        const float den = (float)pose_slot_den(sw, s, p.B, p.n_pts, &fac);
+        return p.gw[__popc(mask & ((1u << s) - 1u))] * (float)fac / den;
+    };
+    float* part = p.part + (long)b * GDRN_POSE_SLOTS;
+    float g[16], GR[9], GTt[3] = {0.f, 0.f, 0.f}, d[3];
+    for (int i = 0; i < 9; ++i) GR[i] = 0.f;
+    for (int k = 0; k < 9; ++k) g[k] = 0.f;
+    // ---- point matching (pm_loss.py:97-171)
+    if (mode != kPmOff) {
+        float c[3] = {0.f, 0.f, 0.f};
+        for (int s = kSlotPmR; s <= kSlotPmZ; ++s) {
+            if (!((mask >> s) & 1u)) continue;
+            if (kind == kLossL2) {
+                const float nrm = sqrtf(sAcc[s]);
+                part[s] = nrm;
+                c[s] = nrm > 0.f ? coef(s) / nrm : 0.f;
+            } else {
+                part[s] = sAcc[s];
+                c[s] = coef(s);
+            }
+        }
+        for (int k = 0; k < 9; ++k) {
+            float s = 0.f;
+            for (int ij = 0; ij < 9; ++ij) s += sG[ij] * sJ[ij][k];
+            g[k] = c[0] * s;
+        }
+        if (mode == kPmRT)
+            for (int i = 0; i < 3; ++i) GTt[i] += c[0] * sGT[i];
+        if (mode == kPmDisT || mode == kPmDisZ)
+            for (int i = 0; i < 3; ++i) GTt[i] += c[(mode == kPmDisZ && i == 2) ? 2 : 1] * sGT[i];
+        // without points: loss_func(t, t_gt) on [B, 3], or on [B, 2] and [B] -- no weights, no factor 3, no PM_LW
+        if (mode == kPmDisTNoP || mode == kPmDisZNoP) {
+            const float e[3] = {Tp[0] - Tg[0], Tp[1] - Tg[1], Tp[2] - Tg[2]};
+            if (mode == kPmDisTNoP) {
+                part[kSlotNoP] = pose_group(kind, beta, e, 3, coef(kSlotNoP), d);
+                for (int i = 0; i < 3; ++i) GTt[i] += d[i];
+            } else {
+                part[kSlotNoP] = pose_group(kind, beta, e, 2, coef(kSlotNoP), d);
+                GTt[0] += d[0];
+                GTt[1] += d[1];
+                part[kSlotNoPZ] = pose_group(kind, beta, e + 2, 1, coef(kSlotNoPZ), d);
+                GTt[2] += d[0];
+            }
+        }
+    }
+    // ---- loss_rot against the original R_gt (rot_loss.py:30-48): angular (1 - (tr(R R_gt^T) - 1) / 2) / 2, or mean (R - R_gt)^2
+    if ((mask >> kSlotRot) & 1u) {
+        const float c = coef(kSlotRot);
+        if (sw.rot_type == 0) {
+            float m[3];
+            for (int i = 0; i < 3; ++i) m[i] = sR[i * 3] * sRg0[i * 3] + sR[i * 3 + 1] * sRg0[i * 3 + 1] + sR[i * 3 + 2] * sRg0[i * 3 + 2];
+            const float cs = (m[0] + m[1] + m[2] - 1.f) / 2.f;
+            part[kSlotRot] = (1.f - cs) / 2.f;
+            for (int i = 0; i < 9; ++i) GR[i] += -0.25f * c * sRg0[i];
+        } else {
+            float s = 0.f;
+            for (int i = 0; i < 9; ++i) {
+                const float e = sR[i] - sRg0[i];
+                s += __fmul_rn(e, e);
+                GR[i] += 2.f * c * e;
+            }
+            part[kSlotRot] = s;
+        }
+    }
+    // ---- centroid and z on the raw network output against trans_ratio (GDRN.py:439-471; L2 of the [B] z is its L1)
+    const float* tp = p.pred_t + (long)b * p.ld_pred;
+    const float* gr = p.gt_ratio + b * 3;
+    const float ec[2] = {tp[0] - gr[0], tp[1] - gr[1]}, ez = tp[2] - gr[2];
+    float dc[2], dz;
+    part[kSlotCentroid] = pose_group(sw.centroid_type, 0.f, ec, 2, coef(kSlotCentroid), dc);
+    part[kSlotZ] = pose_group(sw.z_type, 0.f, &ez, 1, coef(kSlotZ), &dz);
+    // ---- translation (GDRN.py:474-500): xy and z, or all three (loss_trans_LPnP)
+    if ((mask >> kSlotTrans) & 1u) {
+        const float e[3] = {Tp[0] - Tg[0], Tp[1] - Tg[1], Tp[2] - Tg[2]};
+        if (sw.trans_disentangle) {
+            part[kSlotTrans] = pose_group(sw.trans_type, 0.f, e, 2, coef(kSlotTrans), d);
+            GTt[0] += d[0];
+            GTt[1] += d[1];
+            part[kSlotTransZ] = pose_group(sw.trans_type, 0.f, e + 2, 1, coef(kSlotTransZ), d);
+            GTt[2] += d[0];
+        } else {
+            part[kSlotTrans] = pose_group(sw.trans_type, 0.f, e, 3, coef(kSlotTrans), d);
+            for (int i = 0; i < 3; ++i) GTt[i] += d[i];
+        }
+    }
+    // ---- bind (GDRN.py:503-514): R^T t against R_gt^T t_gt (original R_gt)
+    if ((mask >> kSlotBind) & 1u) {
+        float e[3];
+        for (int j = 0; j < 3; ++j) {
+            const float pb = sR[j] * Tp[0] + sR[3 + j] * Tp[1] + sR[6 + j] * Tp[2];
+            const float gb = sRg0[j] * Tg[0] + sRg0[3 + j] * Tg[1] + sRg0[6 + j] * Tg[2];
+            e[j] = pb - gb;
+        }
+        part[kSlotBind] = pose_group(sw.bind_type, 0.f, e, 3, coef(kSlotBind), d);
+        for (int i = 0; i < 3; ++i)
+            for (int j = 0; j < 3; ++j) {
+                GR[i * 3 + j] += Tp[i] * d[j];
+                GTt[i] += sR[i * 3 + j] * d[j];
+            }
+    }
+    // ---- chain rule through the decode; the shipped configuration adds nothing here
+    if ((mask & ~((1u << kSlotPmR) | (1u << kSlotCentroid) | (1u << kSlotZ))) != 0u || mode == kPmRT) {
+        for (int k = 0; k < 9; ++k) {
+            float s = 0.f;
+            for (int ij = 0; ij < 9; ++ij) s += GR[ij] * sJ[ij][k];
+            for (int i = 0; i < 3; ++i) s += GTt[i] * sJT[i][k];
+            g[k] += s;
+        }
+    }
+    g[6] += dc[0];
+    g[7] += dc[1];
+    g[8] += dz;
+    for (int k = 9; k < 16; ++k) g[k] = 0.f;
+    for (int k = 0; k < 64; k += 2) {
+        const float a = k < 16 ? g[k] : 0.f, c = k + 1 < 16 ? g[k + 1] : 0.f;
+        uint32_t h, l;
+        split2(a, c, h, l);
+        *reinterpret_cast<uint32_t*>(p.dy_hi + (long)b * 64 + k) = h;
+        if (p.dy_lo != nullptr) *reinterpret_cast<uint32_t*>(p.dy_lo + (long)b * 64 + k) = l;
+    }
+}
+
+// EX = false: the shipped configuration (r_only L1 PM normalised by extent, L1 centroid and z) with atomic fp64 sums;
+// EX = true: every PNP_NET switch (gdrn_pose_switches), per-crop partials.  Both share the decode and the symmetric search.
+template <bool EX>
 __global__ void __launch_bounds__(128) pose_loss_kernel(const PoseParams p) {
     const int b = blockIdx.x;
     __shared__ float sR[9], sRgt[9], sG[9], sT[3];
     __shared__ float sJ[9][9];  // dR[i][j]/d input k
-    __shared__ float red[10][4];
+    __shared__ float red[EX ? 15 : 10][4];
+    __shared__ float sJT[3][9], sRg0[9], sGT[3], sAcc[3];  // EX: dT[i]/d input k, the original (not symmetric) R_gt
     if (threadIdx.x == 0) {
         const float* r6 = p.rot6d + (long)b * p.ld_pred;
         const float* tp = p.pred_t + (long)b * p.ld_pred;
@@ -523,6 +822,8 @@ __global__ void __launch_bounds__(128) pose_loss_kernel(const PoseParams p) {
         for (int i = 0; i < 3; ++i) {
             sT[i] = T[i].v;
             p.out_trans[b * 3 + i] = T[i].v;
+            if (EX)
+                for (int k = 0; k < 9; ++k) sJT[i][k] = T[i].d[k];
         }
         if (p.do_loss) {
             // ground-truth rotation, optionally replaced by the closest symmetric equivalent (detached)
@@ -545,6 +846,8 @@ __global__ void __launch_bounds__(128) pose_loss_kernel(const PoseParams p) {
                 p.vis[b * 2 + 1] = (float)sqrt(te);
             }
             for (int i = 0; i < 9; ++i) sRgt[i] = Rg[i];
+            if (EX)
+                for (int i = 0; i < 9; ++i) sRg0[i] = Rg[i];
         }
     }
     __syncthreads();
@@ -617,6 +920,11 @@ __global__ void __launch_bounds__(128) pose_loss_kernel(const PoseParams p) {
             }
         }
         __syncthreads();
+    }
+
+    if constexpr (EX) {
+        pose_loss_ex_tail(p, sR, sRgt, sRg0, sT, sJ, sJT, sG, sGT, sAcc, red);
+        return;
     }
 
     // point-matching loss (r_only, L1, normalised by max extent): sum |w (R p - Rgt p)|, and dL/dR = w sign(e) p^T
@@ -704,6 +1012,37 @@ __global__ void loss_finalize_kernel(const double* __restrict__ pix_sums, const 
     losses[5] = (float)(pose_sums[0] / ((double)B * n_pts));
     losses[6] = (float)(pose_sums[1] / (2.0 * B));
     losses[7] = (float)(pose_sums[2] / (double)B);
+    float re = 0.f, te = 0.f;
+    for (int b = 0; b < B; ++b) {
+        re += vis[b * 2];
+        te += vis[b * 2 + 1];
+    }
+    vis_out[0] = re / B;
+    vis_out[1] = te / B;
+}
+
+// losses[5 + n_pose]: the pixel losses as loss_finalize_kernel (region normaliser slot 6), then each active pose slot as the
+// crop-ordered fp64 sum of its partials (no atomics: the same inputs give the same losses)
+__global__ void loss_finalize_ex2_kernel(const double* __restrict__ pix_sums, const float* __restrict__ part,
+                                         const float* __restrict__ vis, float* __restrict__ losses, float* __restrict__ vis_out,
+                                         int B, int HW, int n_pts, const gdrn_pose_switches sw) {
+    if (threadIdx.x != 0 || blockIdx.x != 0) return;
+    const double fg = pix_sums[5] < 1.0 ? 1.0 : pix_sums[5];
+    const double fg_reg = pix_sums[6] < 1.0 ? 1.0 : pix_sums[6];
+    losses[0] = (float)(pix_sums[0] / fg);
+    losses[1] = (float)(pix_sums[1] / fg);
+    losses[2] = (float)(pix_sums[2] / fg);
+    losses[3] = (float)(pix_sums[3] / ((double)B * HW));
+    losses[4] = (float)(pix_sums[4] / fg_reg);
+    const unsigned mask = pose_slot_mask(sw);
+    int o = 5;
+    for (int s = 0; s < GDRN_POSE_SLOTS; ++s) {
+        if (!((mask >> s) & 1u)) continue;
+        double sum = 0.0, fac;
+        for (int b = 0; b < B; ++b) sum += (double)part[(long)b * GDRN_POSE_SLOTS + s];
+        const double den = pose_slot_den(sw, s, B, n_pts, &fac);
+        losses[o++] = (float)(fac == 1.0 ? sum / den : fac * sum / den);
+    }
     float re = 0.f, te = 0.f;
     for (int b = 0; b < B; ++b) {
         re += vis[b * 2];
@@ -888,7 +1227,71 @@ extern "C" int gdrn_pose_loss(const float* pred, int ld_pred, const float* cams,
     p.do_loss = do_loss;
     p.eps = eps;
     if (do_loss) GDRN_CUDA_OK(cudaMemsetAsync(sums, 0, 4 * sizeof(double), stream));
-    pose_loss_kernel<<<B, 128, 0, stream>>>(p);
+    pose_loss_kernel<false><<<B, 128, 0, stream>>>(p);
+    GDRN_CUDA_OK(cudaGetLastError());
+    count_launch();
+    return 0;
+}
+
+static int check_pose_switches(const char* fn, const gdrn_pose_switches& sw) {
+    const auto kind3 = [](int t) { return t == kLossL1 || t == kLossMSE || t == kLossL2; };  // L1 | MSE | L2
+    if (sw.pm_mode < kPmOff || sw.pm_mode > kPmDisZNoP) return set_error(GDRN_ERR_ARG, "%s: pm_mode %d", fn, sw.pm_mode);
+    if (sw.pm_type < kLossL1 || sw.pm_type > kLossL2) return set_error(GDRN_ERR_ARG, "%s: pm_type %d", fn, sw.pm_type);
+    if (sw.rot_type < -1 || sw.rot_type > 1) return set_error(GDRN_ERR_ARG, "%s: rot_type %d", fn, sw.rot_type);
+    if (!kind3(sw.centroid_type) || !kind3(sw.z_type)) return set_error(GDRN_ERR_ARG, "%s: centroid / z loss type", fn);
+    if ((sw.trans_type != -1 && !kind3(sw.trans_type)) || (sw.bind_type != -1 && !kind3(sw.bind_type)))
+        return set_error(GDRN_ERR_ARG, "%s: trans / bind loss type", fn);
+    return 0;
+}
+
+extern "C" int gdrn_pose_loss_count(gdrn_pose_switches sw) { return __builtin_popcount(pose_slot_mask(sw)); }
+
+extern "C" int gdrn_pose_loss_ex(const float* pred, int ld_pred, const float* cams, const float* centers, const float* whs,
+                                 const float* ratios, const float* extents, const float* points, const float* gt_rot,
+                                 const float* gt_trans, const float* gt_ratio, const float* syms, const int* sym_idx,
+                                 const float* gw, float* out_rot, float* out_trans, float* part, float* vis, void* dy_hi,
+                                 void* dy_lo, int B, int n_pts, gdrn_pose_switches sw, void* stream_) {
+    if (int rc = check_pose_switches("pose_loss_ex", sw)) return rc;
+    if (part == nullptr || gw == nullptr || points == nullptr) return set_error(GDRN_ERR_ARG, "pose_loss_ex: part, gw and points are required");
+    PoseParams p;
+    p.rot6d = pred;
+    p.pred_t = pred + 6;
+    p.ld_pred = ld_pred;
+    p.cams = cams;
+    p.centers = centers;
+    p.whs = whs;
+    p.ratios = ratios;
+    p.extents = extents;
+    p.points = points;
+    p.gt_rot = gt_rot;
+    p.gt_trans = gt_trans;
+    p.gt_ratio = gt_ratio;
+    p.syms = syms;
+    p.sym_idx = sym_idx;
+    p.gw = gw;
+    p.out_rot = out_rot;
+    p.out_trans = out_trans;
+    p.sums = nullptr;
+    p.vis = vis;
+    p.dy_hi = (bf16*)dy_hi;
+    p.dy_lo = (bf16*)dy_lo;
+    p.B = B;
+    p.n_pts = n_pts;
+    p.do_loss = 1;
+    p.eps = 1e-4f;
+    p.sw = sw;
+    p.part = part;
+    pose_loss_kernel<true><<<B, 128, 0, reinterpret_cast<cudaStream_t>(stream_)>>>(p);
+    GDRN_CUDA_OK(cudaGetLastError());
+    count_launch();
+    return 0;
+}
+
+extern "C" int gdrn_loss_finalize_ex2(const double* pix_sums, const float* part, const float* vis, float* losses, float* vis_out,
+                                      int B, int HW, int n_pts, gdrn_pose_switches sw, void* stream_) {
+    if (int rc = check_pose_switches("loss_finalize_ex2", sw)) return rc;
+    loss_finalize_ex2_kernel<<<1, 32, 0, reinterpret_cast<cudaStream_t>(stream_)>>>(pix_sums, part, vis, losses, vis_out, B, HW,
+                                                                                     n_pts, sw);
     GDRN_CUDA_OK(cudaGetLastError());
     count_launch();
     return 0;

@@ -28,6 +28,70 @@ LOSS_NAMES = ["loss_coor_x", "loss_coor_y", "loss_coor_z", "loss_mask", "loss_re
 MASK_LOSSES = {"L1": 0, "BCE": 1, "CE": 2}  # ROT_HEAD.MASK_LOSS_TYPE -> the mask_loss argument of the gdrn_*_ex loss kernels
 HEAD_CONVS = [(3, 4, False), (6, 7, False), (10, 11, True), (13, 14, False), (17, 18, True), (20, 21, False)]
 
+# PNP_NET pose-loss switches -> gdrn_pose_switches (include/gdrn_b200.h)
+POSE_LOSS_KINDS = {"l1": 0, "smooth_l1": 1, "mse": 2, "l2": 3}  # PM_LOSS_TYPE, lower-cased like PyPMLoss (pm_loss.py:70)
+POSE_LOSS_KINDS3 = {"L1": 0, "MSE": 2, "L2": 3}  # CENTROID / Z / TRANS / BIND_LOSS_TYPE (GDRN.py:439-514)
+PM_MODES = {"off": -1, "R": 0, "RT": 1, "T": 2, "Z": 3, "T_noP": 4, "Z_noP": 5}
+DEFAULT_POSE_SWITCHES = dict(pm_mode=0, pm_type=0, pm_norm_extent=1, rot_type=-1, centroid_type=0, z_type=0, trans_type=-1,
+                             trans_disentangle=1, bind_type=-1)
+
+
+def pose_loss_switches(pnp_cfg) -> tuple:
+    """(switches dict, the pose-side loss names in loss_dict order) of a PNP_NET config; raises ValueError naming the offending key.
+    PyPMLoss (pm_loss.py:58-171): R_ONLY wins, DISENTANGLE_Z implies DISENTANGLE_T, without either t joins the points.  The
+    centroid and z losses are always computed (GDRN.forward drops them when their weight is 0)."""
+    p = pnp_cfg
+    sw = dict(DEFAULT_POSE_SWITCHES, pm_beta=float(p.get("PM_SMOOTH_L1_BETA", 1.0)), pm_norm_extent=int(bool(p.PM_NORM_BY_EXTENT)))
+    names = []
+    pm_type = str(p.PM_LOSS_TYPE).lower()
+    if pm_type not in POSE_LOSS_KINDS:
+        raise ValueError(f"PNP_NET.PM_LOSS_TYPE = {p.PM_LOSS_TYPE!r} (L1, Smooth_L1, MSE or L2)")
+    sw["pm_type"] = POSE_LOSS_KINDS[pm_type]
+    if p.PM_LW <= 0:
+        mode = "off"
+    elif p.PM_R_ONLY:
+        mode, names = "R", ["loss_PM_R"]
+    elif p.PM_DISENTANGLE_Z:
+        mode = "Z" if p.PM_T_USE_POINTS else "Z_noP"
+        names = ["loss_PM_R", "loss_PM_xy", "loss_PM_z"] if p.PM_T_USE_POINTS else ["loss_PM_R", "loss_PM_xy_noP", "loss_PM_z_noP"]
+    elif p.PM_DISENTANGLE_T:
+        mode = "T" if p.PM_T_USE_POINTS else "T_noP"
+        names = ["loss_PM_R", "loss_PM_T"] if p.PM_T_USE_POINTS else ["loss_PM_R", "loss_PM_T_noP"]
+    else:
+        mode, names = "RT", ["loss_PM_RT"]
+    sw["pm_mode"] = PM_MODES[mode]
+
+    def kind3(key):
+        v = p.get(key, "L1")
+        if v not in POSE_LOSS_KINDS3:
+            raise ValueError(f"PNP_NET.{key} = {v!r} (L1, L2 or MSE)")
+        return POSE_LOSS_KINDS3[v]
+
+    if p.ROT_LW > 0:
+        if p.ROT_LOSS_TYPE not in ("angular", "L2"):
+            raise ValueError(f"PNP_NET.ROT_LOSS_TYPE = {p.ROT_LOSS_TYPE!r} (angular or L2)")
+        sw["rot_type"] = 0 if p.ROT_LOSS_TYPE == "angular" else 1
+        names.append("loss_rot")
+    sw["centroid_type"] = kind3("CENTROID_LOSS_TYPE") if p.CENTROID_LW > 0 else 0
+    sw["z_type"] = kind3("Z_LOSS_TYPE") if p.Z_LW > 0 else 0
+    names += ["loss_centroid", "loss_z"]
+    if p.TRANS_LW > 0:
+        sw["trans_type"] = kind3("TRANS_LOSS_TYPE")
+        sw["trans_disentangle"] = int(bool(p.TRANS_LOSS_DISENTANGLE))
+        names += ["loss_trans_xy", "loss_trans_z"] if p.TRANS_LOSS_DISENTANGLE else ["loss_trans_LPnP"]
+    if p.get("BIND_LW", 0.0) > 0:
+        # GDRN.py:505-512: L1, L2, else MSE when CENTROID_LOSS_TYPE (sic) is "MSE", else a ValueError
+        bt = p.get("BIND_LOSS_TYPE", "L1")
+        if bt in ("L1", "L2"):
+            sw["bind_type"] = POSE_LOSS_KINDS3[bt]
+        elif p.CENTROID_LOSS_TYPE == "MSE":
+            sw["bind_type"] = POSE_LOSS_KINDS3["MSE"]
+        else:
+            raise ValueError(f"PNP_NET.BIND_LOSS_TYPE = {bt!r} (L1 or L2, or anything with CENTROID_LOSS_TYPE = 'MSE', which then "
+                             "selects MSE)")
+        names.append("loss_bind")
+    return sw, names
+
 
 class _BN:
     """Per-BatchNorm scratch: scale/shift (forward), mean/invstd (backward), statistic slices."""
@@ -123,6 +187,15 @@ class Engine:
         self.mask_out = model.rot_head_net.features[23].out_channels - 68  # mask | xyz | bg + 64 regions
         assert self.mask_out == (2 if self.mask_loss == MASK_LOSSES["CE"] else 1), (self.mask_loss, self.mask_out)
         self.mask_gt = (rh.XYZ_LOSS_MASK_GT, rh.MASK_LOSS_GT, rh.REGION_LOSS_MASK_GT)
+        # pose losses (PNP_NET switches): the shipped set runs gdrn_pose_loss (8 losses, LOSS_NAMES), any other gdrn_pose_loss_ex
+        sw, pose_names = pose_loss_switches(model.cfg.MODEL.CDPN.PNP_NET)
+        self.loss_names = LOSS_NAMES[:5] + pose_names
+        self.pose_ex = any(sw[k] != v for k, v in DEFAULT_POSE_SWITCHES.items())
+        from .capi import PoseSwitches
+
+        self.pose_sw = PoseSwitches(**sw)
+        assert self.pose_ex or self.loss_names == LOSS_NAMES, self.loss_names
+        assert int(C.load().gdrn_pose_loss_count(self.pose_sw)) == len(pose_names), (sw, pose_names)
         self.named_params = list(model.named_parameters())
         self.bn: Dict[str, _BN] = {}
         total = 0
@@ -156,7 +229,9 @@ class Engine:
         # fp16 planes: activation gradients are carried with a static power-of-two loss scale (exactly removed from the
         # fp32 parameter gradients at the end of backward), like the GradScaler of the reference's AMP configs
         self.storage_name = ops.storage_format()[2]
-        self.grad_scale = 1024.0 if self.storage_name == "fp16" else 1.0
+        # The pose-loss switches bring gradients up to ~sqrt(n) w / B per unit loss (L2 point matching: 2e2 at n = 3000, B = 4),
+        # which overflow fp16 at 1024; 64 keeps them in range and the smallest (mask channel, 1 / (B 4096) at B = 64) normal.
+        self.grad_scale = (64.0 if self.pose_ex else 1024.0) if self.storage_name == "fp16" else 1.0
         from .dist import SEGMENTS, segment_bounds
 
         self._seg = segment_bounds(self.named_params, SEGMENTS)
@@ -557,11 +632,15 @@ class Engine:
         # the pose kernel needs the upstream loss gradients to emit dY9; forward calls it with unit weights and
         # backward re-runs it (cheap: B CTAs) with the actual ones.
         self._pose(S, gw=None)
-        losses = torch.empty(8, device=dev)
+        losses = torch.empty(len(self.loss_names), device=dev)
         vis2 = torch.empty(2, device=dev)
         n_pts = aux["gt_points"].shape[1]
-        C.gdrn_loss_finalize_ex(pix_sums.data_ptr(), S["pose_sums"].data_ptr(), S["vis_ps"].data_ptr(), losses.data_ptr(),
-                                vis2.data_ptr(), B, 4096, n_pts, _stream())
+        if self.pose_ex:
+            C.gdrn_loss_finalize_ex2(pix_sums.data_ptr(), S["pose_part"].data_ptr(), S["vis_ps"].data_ptr(), losses.data_ptr(),
+                                     vis2.data_ptr(), B, 4096, n_pts, self.pose_sw, _stream())
+        else:
+            C.gdrn_loss_finalize_ex(pix_sums.data_ptr(), S["pose_sums"].data_ptr(), S["vis_ps"].data_ptr(), losses.data_ptr(),
+                                    vis2.data_ptr(), B, 4096, n_pts, _stream())
         vis = torch.cat([vis2, S["out_trans"][0], pred[0, 6:9], aux["gt_trans"][0], aux["gt_trans_ratio"][0]])
         return dict(rot=S["out_rot"], trans=S["out_trans"], pred=pred, losses=losses, vis=vis, logits=logits)
 
@@ -581,7 +660,10 @@ class Engine:
         if "out_rot" not in S:
             S["out_rot"] = torch.empty(B, 3, 3, device=dev)
             S["out_trans"] = torch.empty(B, 3, device=dev)
-            S["pose_sums"] = torch.empty(4, dtype=torch.float64, device=dev)
+            if self.pose_ex:
+                S["pose_part"] = torch.empty(B, 11, device=dev)  # [B][GDRN_POSE_SLOTS] per-crop partials
+            else:
+                S["pose_sums"] = torch.empty(4, dtype=torch.float64, device=dev)
             S["vis_ps"] = torch.empty(B, 2, device=dev)
             S["dy9"] = PT((B, 64), self.bplanes, device=dev)
         sym_idx = aux.get("sym_idx")
@@ -589,8 +671,16 @@ class Engine:
             sym_idx = aux["sym_idx"] = self.sym_table.indices(aux["sym_infos"])
         syms = self.sym_table.table if sym_idx is not None else None
         if gw is None:
-            gw = torch.ones(3, device=dev)
+            gw = torch.ones(len(self.loss_names) - 5, device=dev)
         n_pts = aux["gt_points"].shape[1]
+        if self.pose_ex:
+            C.gdrn_pose_loss_ex(S["pred"].data_ptr(), 16, aux["roi_cams"].data_ptr(), aux["roi_centers"].data_ptr(),
+                                aux["roi_whs"].data_ptr(), aux["resize_ratios"].data_ptr(), aux["roi_extents"].data_ptr(),
+                                aux["gt_points"].data_ptr(), aux["gt_ego_rot"].data_ptr(), aux["gt_trans"].data_ptr(),
+                                aux["gt_trans_ratio"].data_ptr(), ops.ptr(syms), ops.ptr(sym_idx), gw.data_ptr(),
+                                S["out_rot"].data_ptr(), S["out_trans"].data_ptr(), S["pose_part"].data_ptr(), S["vis_ps"].data_ptr(),
+                                S["dy9"].hi_ptr, S["dy9"].lo_ptr, B, n_pts, self.pose_sw, _stream())
+            return
         C.gdrn_pose_loss(S["pred"].data_ptr(), 16, aux["roi_cams"].data_ptr(), aux["roi_centers"].data_ptr(),
                          aux["roi_whs"].data_ptr(), aux["resize_ratios"].data_ptr(), aux["roi_extents"].data_ptr(),
                          aux["gt_points"].data_ptr(), aux["gt_ego_rot"].data_ptr(), aux["gt_trans"].data_ptr(),
@@ -646,7 +736,8 @@ class Engine:
                           det_ws=self._det_workspace() if self.deterministic else None)
 
     def backward(self, grad_losses: torch.Tensor):
-        """grad_losses: [8] upstream gradients of LOSS_NAMES.  Fills self.grads (views of self.flat_grad)."""
+        """grad_losses: upstream gradients of self.loss_names ([8], LOSS_NAMES, by default).  Fills self.grads (views of
+        self.flat_grad)."""
         S, m, dev = self.saved, self.model, self.dev
         assert S is not None, "backward called without a do_loss forward"
         B, aux, pn = S["B"], S["aux"], m.pnp_net
@@ -660,7 +751,7 @@ class Engine:
         gw = grad_losses.float().contiguous()
         if self.grad_scale != 1.0:
             gw = gw * self.grad_scale  # the whole backward is linear in the loss gradients
-        self._pose(S, gw=gw[5:8].contiguous())
+        self._pose(S, gw=gw[5:].contiguous())
         dy9 = S["dy9"]
         tmp = torch.empty(1024, device=dev)
 
@@ -863,7 +954,7 @@ class GraphedTrainStep:
         if self.aux.get("sym_infos") is not None:  # symmetric PM: only the (first row, count) pairs are a per-step input
             self.aux["sym_idx"] = engine.sym_table.indices(self.aux["sym_infos"])
         self.aux.pop("sym_infos", None)
-        self.gw = torch.ones(8, device=x.device)
+        self.gw = torch.ones(len(engine.loss_names), device=x.device)
 
         def one_step():
             res = engine.forward(self.x, self.aux, train_bn=train_bn, do_loss=True)
@@ -895,7 +986,7 @@ class GraphedFwdBwd:
     def __init__(self, engine: "Engine", x: torch.Tensor, aux: dict, train_bn: bool):
         self.engine, self.train_bn = engine, train_bn
         self.x, self.aux = _clone_inputs(x, aux)
-        self.gw = torch.ones(8, device=x.device)
+        self.gw = torch.ones(len(engine.loss_names), device=x.device)
         self.key = self.signature(x, aux, train_bn)
 
         def bwd():

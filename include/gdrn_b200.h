@@ -185,6 +185,32 @@ int gdrn_loss_finalize(const double* pix_sums, const double* pose_sums, const fl
 int gdrn_loss_finalize_ex(const double* pix_sums, const double* pose_sums, const float* vis, float* losses, float* vis_out,
                           int B, int HW, int n_pts, void* stream);
 
+/* ---- the PNP_NET pose-loss switches (GDRN.py:402-514, pm_loss.py:58-171, rot_loss.py:30-48, l2_loss.py), passed by value.
+ * Loss kinds: 0 L1, 1 Smooth-L1 (PM only, fvcore: plain L1 for beta < 1e-5), 2 MSE, 3 L2 (per-crop norm, mean over B).
+ * pm_mode: -1 no PM loss (PM_LW = 0), 0 R only, 1 R and t together (loss_PM_RT), 2 DISENTANGLE_T with points (PM_R, PM_T),
+ * 3 DISENTANGLE_Z with points (PM_R, PM_xy, PM_z), 4 DISENTANGLE_T without points (PM_R, PM_T_noP), 5 DISENTANGLE_Z without
+ * points (PM_R, PM_xy_noP, PM_z_noP).  rot_type: -1 off, 0 angular, 1 L2.  trans_type, bind_type: -1 off, else L1 / MSE / L2.
+ * The default (pm_mode 0, L1, norm by extent, centroid and z L1, the rest off) is what gdrn_pose_loss computes. */
+typedef struct {
+    int pm_mode, pm_type;
+    float pm_beta;
+    int pm_norm_extent, rot_type, centroid_type, z_type, trans_type, trans_disentangle, bind_type;
+} gdrn_pose_switches;
+#define GDRN_POSE_SLOTS 11 /* per-crop partial sums: PM R|RT, PM T|xy, PM z, PM T_noP|xy_noP, PM z_noP, rot, centroid, z,
+                              trans xy|LPnP, trans z, bind; the active ones, in this order, are the reference's loss_dict order */
+/* gdrn_pose_loss with the switches: part [B][GDRN_POSE_SLOTS] per-crop partial sums (inactive slots unwritten); gw: the upstream
+ * gradients of the ACTIVE pose losses in slot order; dy as gdrn_pose_loss. */
+int gdrn_pose_loss_ex(const float* pred, int ld_pred, const float* cams, const float* centers, const float* whs,
+                      const float* ratios, const float* extents, const float* points, const float* gt_rot,
+                      const float* gt_trans, const float* gt_ratio, const float* syms, const int* sym_idx, const float* gw,
+                      float* out_rot, float* out_trans, float* part, float* vis, void* dy_hi, void* dy_lo, int B, int n_pts,
+                      gdrn_pose_switches sw, void* stream);
+/* losses[5 + n_pose] = the five pixel losses (as gdrn_loss_finalize_ex) then the active pose losses in slot order, each the
+ * crop-ordered sum of its partials (deterministic); n_pose = gdrn_pose_loss_count(sw) */
+int gdrn_loss_finalize_ex2(const double* pix_sums, const float* part, const float* vis, float* losses, float* vis_out, int B,
+                           int HW, int n_pts, gdrn_pose_switches sw, void* stream);
+int gdrn_pose_loss_count(gdrn_pose_switches sw);
+
 /* ---- per-instance crop / target generation of the data loader on the device (core/gdrn_modeling/data_loader.py:487-560,
  * core/utils/data_utils.py:80-137 crop_resize_by_warp_affine, :213-219 xyz_to_region), cv2.warpAffine's fixed-point sampling
  * restated.  image_u8 [B][H][W][3] (BGR uint8), centers [B][2], scales [B] (float64 like the reference's aug_bbox output) -> roi_img [B][3][R][R] = bilinear crop / pixel_std.
