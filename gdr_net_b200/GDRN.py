@@ -154,7 +154,7 @@ class ConvPnPNet(_ParamsOnly):
 
     def forward(self, coor_feat, region=None, extents=None, mask_attention=None):
         """Stand-alone Patch-PnP inference with the reference signature (conv_pnp_net.py:111): xyz(+2-D coords) maps
-        [B, 3|5, 64, 64], region attention [B, 64, 64, 64], extents [B, 3] -> (rot [B, rot_dim], t [B, 3]).
+        [B, 3|5, 64, 64], region attention [B, R, 64, 64] or None, extents [B, 3] -> (rot [B, rot_dim], t [B, 3]).
         Runs patch_pnp.PatchPnP (libgdrn_b200.so kernels, one CUDA graph); no autograd, no CPU fallback.  Inside
         `GDRN.forward` the engine runs the same kernels with the hand-written backward instead."""
         if mask_attention is not None:
@@ -195,14 +195,18 @@ def _check_supported(cfg):
         problems.append("backbone must be resnet18/34 at 256 -> 64")
     if r.ROT_CONCAT or r.ROT_CLASS_AWARE or r.MASK_CLASS_AWARE or r.REGION_CLASS_AWARE:
         problems.append("class-aware / concat heads")
-    if r.XYZ_LOSS_TYPE != "L1" or r.MASK_LOSS_TYPE not in ("L1", "BCE", "CE") or r.REGION_LOSS_TYPE != "CE" or r.NUM_REGIONS != 64:
-        problems.append("losses other than xyz L1 / mask L1, BCE or CE / region CE over 64 regions")
+    if r.XYZ_LOSS_TYPE != "L1" or r.MASK_LOSS_TYPE not in ("L1", "BCE", "CE") or r.REGION_LOSS_TYPE != "CE":
+        problems.append("losses other than xyz L1 / mask L1, BCE or CE / region CE")
+    # the per-pixel kernels hold a logit row of 72 floats: MO + 3 + (R + 1) <= 70 for R <= 64; R < 2 fails the reference's own
+    # region_out_dim > 2 assert (GDRN.py:546)
+    if not 2 <= r.NUM_REGIONS <= 64:
+        problems.append(f"ROT_HEAD.NUM_REGIONS = {r.NUM_REGIONS!r} (2..64)")
     # gdrn_loss builds gt_masks = {"trunc", "visib", "obj"} (GDRN.py:339); any other key (the config comment's "gt") is a KeyError there
     for key in ("XYZ_LOSS_MASK_GT", "MASK_LOSS_GT", "REGION_LOSS_MASK_GT"):
         if getattr(r, key) not in ("trunc", "visib", "obj"):
             problems.append(f"ROT_HEAD.{key} = {getattr(r, key)!r} (trunc, visib or obj)")
-    if not p.REGION_ATTENTION or p.MASK_ATTENTION != "none" or p.R_ONLY:
-        problems.append("Patch-PnP input other than xyz (+ 2D coords) + region attention (PNP_NET.REGION_ATTENTION, MASK_ATTENTION, R_ONLY)")
+    if p.MASK_ATTENTION != "none" or p.R_ONLY:
+        problems.append("Patch-PnP input other than xyz (+ 2D coords) (+ region attention) (PNP_NET.MASK_ATTENTION, R_ONLY)")
     if p.ROT_TYPE != "allo_rot6d" or p.TRANS_TYPE != "centroid_z" or p.Z_TYPE != "REL":
         problems.append(f"pose parametrisation other than allo_rot6d + centroid_z(REL) (PNP_NET.ROT_TYPE = {p.ROT_TYPE!r}, "
                         f"TRANS_TYPE = {p.TRANS_TYPE!r}, Z_TYPE = {p.Z_TYPE!r})")

@@ -178,13 +178,22 @@ class Engine:
         self.deterministic = os.environ.get("GDRN_DETERMINISTIC", "1") == "1"
         self._det_ws = None
         self.fold_eval = True  # inference by forward_eval_folded; False runs it through the unfused train-path kernels
-        self.with_2d = int(model.pnp_net.features[0].in_channels == 69)  # 69 = xyz + coord2d + regions, 67 without coords
-        assert model.pnp_net.features[0].in_channels in (67, 69), model.pnp_net.features[0].in_channels
+        # surface regions (ROT_HEAD.NUM_REGIONS = R) and the Patch-PnP input (GDRN.py:156-181): xyz | coord2d (WITH_2D_COORD) |
+        # softmax over the R region logits (REGION_ATTENTION), nIn channels in rows of pnp_ld = round_up(nIn, 64)
+        rh = model.cfg.MODEL.CDPN.ROT_HEAD
+        self.num_regions = int(rh.NUM_REGIONS)
+        self.region_att = int(bool(model.cfg.MODEL.CDPN.PNP_NET.REGION_ATTENTION))
+        n_in = model.pnp_net.features[0].in_channels
+        self.with_2d = int(n_in - 3 - self.region_att * self.num_regions == 2)
+        assert n_in == 3 + 2 * self.with_2d + self.region_att * self.num_regions, (n_in, self.num_regions, self.region_att)
+        self.pnp_ld = -(-n_in // 64) * 64
+        # the shipped head (64 regions with attention) runs the gdrn_*_ex loss kernels, every other one the gdrn_*_ex2 ones
+        self.regions_ex2 = not (self.num_regions == 64 and self.region_att)
         # mask head (GDRN.py:339-400): MASK_LOSS_TYPE, the mask logits per pixel (1, or 2 for CE) and the GT mask of the xyz, mask
         # and region losses (XYZ_LOSS_MASK_GT, MASK_LOSS_GT, REGION_LOSS_MASK_GT)
-        rh = model.cfg.MODEL.CDPN.ROT_HEAD
         self.mask_loss = MASK_LOSSES[rh.MASK_LOSS_TYPE]
-        self.mask_out = model.rot_head_net.features[23].out_channels - 68  # mask | xyz | bg + 64 regions
+        self.n_logits = model.rot_head_net.features[23].out_channels  # mask | xyz | bg | R regions
+        self.mask_out = self.n_logits - 4 - self.num_regions
         assert self.mask_out == (2 if self.mask_loss == MASK_LOSSES["CE"] else 1), (self.mask_loss, self.mask_out)
         self.mask_gt = (rh.XYZ_LOSS_MASK_GT, rh.MASK_LOSS_GT, rh.REGION_LOSS_MASK_GT)
         # pose losses (PNP_NET switches): the shipped set runs gdrn_pose_loss (8 losses, LOSS_NAMES), any other gdrn_pose_loss_ex
@@ -414,15 +423,19 @@ class Engine:
 
     def _head_pnp(self, head_in: PT, aux: dict, pnp_saved: Optional[list] = None):
         """1x1 output conv -> glue -> Patch-PnP (GDRN.py:156-181, conv_pnp_net.py:111-157).  Returns the fp32 logits
-        [B*4096, 72] (68 + mask_out valid), the Patch-PnP input planes, pred [B, 16] (cols 0..5 rot6d, 6..8 centroid dx, dy and z) and the inputs
+        [B*4096, 72] (n_logits valid), the Patch-PnP input planes [B, 64, 64, pnp_ld], pred [B, 16] (cols 0..5 rot6d, 6..8 centroid dx, dy and z) and the inputs
         of the three FC layers; pnp_saved receives the Patch-PnP conv activations (pnp_net_forward)."""
         m, B, dev = self.model, head_in.shape[0], self.dev
         logits = torch.empty(B * 4096, 72, device=dev)
-        ops.conv_fwd(head_in, self.wf["rot_head_net.features.23"], 68 + self.mask_out, 1, 1, 1, 0, out_f32=logits,
+        ops.conv_fwd(head_in, self.wf["rot_head_net.features.23"], self.n_logits, 1, 1, 1, 0, out_f32=logits,
                      bias=m.rot_head_net.features[23].bias, ldc=72, want_planes=False)
-        pnp_in = PT((B, 64, 64, 128), self.planes, device=dev)
-        C.gdrn_head_glue_fwd_ex(logits.data_ptr(), ops.ptr(aux.get("roi_coord_2d")), aux["roi_extents"].data_ptr(), pnp_in.hi_ptr,
-                                pnp_in.lo_ptr, B, 4096, self.with_2d, self.mask_out, _stream())
+        pnp_in = PT((B, 64, 64, self.pnp_ld), self.planes, device=dev)
+        glue = (logits.data_ptr(), ops.ptr(aux.get("roi_coord_2d")), aux["roi_extents"].data_ptr(), pnp_in.hi_ptr, pnp_in.lo_ptr, B, 4096,
+                self.with_2d, self.mask_out)
+        if self.regions_ex2:
+            C.gdrn_head_glue_fwd_ex2(*glue, self.num_regions, self.region_att, self.pnp_ld, _stream())
+        else:
+            C.gdrn_head_glue_fwd_ex(*glue, _stream())
         pred = torch.zeros(B, 16, device=dev)
         fc_in = pnp_net_forward(pnp_in, m.pnp_net, self.wf, self.b_rt, pred, pnp_saved)
         return logits, pnp_in, pred, fc_in
@@ -442,7 +455,7 @@ class Engine:
             maps = logits.view(B, 64, 64, 72).permute(0, 3, 1, 2)
             mo = self.mask_out
             res.update(mask=maps[:, 0:mo], coor_x=maps[:, mo:mo + 1], coor_y=maps[:, mo + 1:mo + 2], coor_z=maps[:, mo + 2:mo + 3],
-                       region=maps[:, mo + 3:mo + 68])
+                       region=maps[:, mo + 3:self.n_logits])
         return res
 
     def _prepare_weights_calls(self, need_dgrad: bool):
@@ -451,7 +464,9 @@ class Engine:
         for key, conv in self._conv_modules():
             wf[key] = ops.pack_conv_fwd(conv.weight, pl, out=wf.get(key))
             if need_dgrad:
-                wd[key] = ops.pack_conv_dgrad(conv.weight, bpl, out=wd.get(key))
+                # the logit gradient of head_bwd is 128 columns wide whatever the output conv's row count (MO + 4 + R)
+                ipad = 128 if key == "rot_head_net.features.23" else None
+                wd[key] = ops.pack_conv_dgrad(conv.weight, bpl, out=wd.get(key), ipad=ipad)
         dc = m.rot_head_net.features[0]
         # the ConvTranspose2d forward IS the data gradient of the stride-2 conv whose OIHW weight its IOHW weight is:
         # gdrn_conv_dgrad_s2 evaluates it by output parity over the un-dilated input (no zero-inserted tensor, 1/4 of the MACs)
@@ -624,8 +639,12 @@ class Engine:
         # ---- a5/a6 pose decode + a7..a10 losses
         pix_sums = torch.empty(7, dtype=torch.float64, device=dev)
         m_xyz, m_mask, m_region = self._loss_masks(aux)
-        C.gdrn_pixel_loss_fwd_ex(logits.data_ptr(), aux["gt_xyz"].data_ptr(), m_xyz, m_mask, m_region, aux["gt_region"].data_ptr(),
-                                 pix_sums.data_ptr(), B, 4096, self.mask_loss, self.mask_out, _stream())
+        pix = (logits.data_ptr(), aux["gt_xyz"].data_ptr(), m_xyz, m_mask, m_region, aux["gt_region"].data_ptr(), pix_sums.data_ptr(), B,
+               4096, self.mask_loss, self.mask_out)
+        if self.regions_ex2:
+            C.gdrn_pixel_loss_fwd_ex2(*pix, self.num_regions, self.region_att, self.pnp_ld, _stream())
+        else:
+            C.gdrn_pixel_loss_fwd_ex(*pix, _stream())
         S.update(logits=logits, pnp_in=pnp_in, pnp=pnp_saved, flat=flat, h1=h1, h2=h2, pred=pred, head_in=head_in,
                  pix_sums=pix_sums, aux=aux)
         self.saved = S
@@ -782,18 +801,22 @@ class Engine:
                                  self.grads[f"pnp_net.features.{gi}.bias"], G=pf[gi].num_groups)
             self._wgrad_conv(du, h(L["x_in"]), pf[ci], f"pnp_net.features.{ci}.weight")
             g = self._dgrad_conv(du, pf[ci], f"pnp_net.features.{ci}")
-        d_pnp_in = g  # [B,64,64,128]
+        d_pnp_in = g  # [B,64,64,pnp_ld]
         self._segment_done("pnp_net")
 
         # ---- glue + per-pixel losses backward (one fused pass over the logits)
         dlog = PT((B * 4096, 128), bp, device=dev)
         m_xyz, m_mask, m_region = self._loss_masks(aux)
-        C.gdrn_head_bwd_ex(S["logits"].data_ptr(), aux["gt_xyz"].data_ptr(), m_xyz, m_mask, m_region, aux["gt_region"].data_ptr(),
-                           S["pix_sums"].data_ptr(), gw.data_ptr(), d_pnp_in.hi_ptr, d_pnp_in.lo_ptr, aux["roi_extents"].data_ptr(),
-                           dlog.hi_ptr, dlog.lo_ptr, B, 4096, self.with_2d, self.mask_loss, self.mask_out, _stream())
+        hb = (S["logits"].data_ptr(), aux["gt_xyz"].data_ptr(), m_xyz, m_mask, m_region, aux["gt_region"].data_ptr(),
+              S["pix_sums"].data_ptr(), gw.data_ptr(), d_pnp_in.hi_ptr, d_pnp_in.lo_ptr, aux["roi_extents"].data_ptr(), dlog.hi_ptr,
+              dlog.lo_ptr, B, 4096, self.with_2d, self.mask_loss, self.mask_out)
+        if self.regions_ex2:
+            C.gdrn_head_bwd_ex2(*hb, self.num_regions, self.region_att, self.pnp_ld, _stream())
+        else:
+            C.gdrn_head_bwd_ex(*hb, _stream())
         hf = m.rot_head_net.features
         head_in = h(S["head_in"])
-        n_out = 68 + self.mask_out  # rows of the 1x1 output conv
+        n_out = self.n_logits  # rows of the 1x1 output conv
         def head_out_wgrad():
             buf, ks, kss = ops.gemm_wgrad(dlog, head_in.view(B * 4096, 256), self.ws)
             ops.unpack_wgrad(buf, self.grads["rot_head_net.features.23.weight"], n_out, 256, 1, 1, 256, ks, kss, 256, 1, 0, 0)

@@ -132,10 +132,11 @@ def pack_conv_fwd(w: torch.Tensor, planes: int, out: PT | None = None, ipad: int
     return out
 
 
-def pack_conv_dgrad(w: torch.Tensor, planes: int, out: PT | None = None) -> PT:
-    """Conv2d OIHW fp32 -> [Cin_pad][KH*KW*Cout_pad], taps flipped: dX = conv(dY (zero-inserted if s2), this)."""
+def pack_conv_dgrad(w: torch.Tensor, planes: int, out: PT | None = None, ipad: int | None = None) -> PT:
+    """Conv2d OIHW fp32 -> [Cin_pad][KH*KW*Cout_pad], taps flipped: dX = conv(dY (zero-inserted if s2), this).  ipad: Cout_pad,
+    the row width of dY (default round_up(Cout, 64))."""
     O, I, KH, KW = w.shape
-    opad, ipad = _round_up(I, 64), _round_up(O, 64)
+    opad, ipad = _round_up(I, 64), ipad or _round_up(O, 64)
     krow = KH * KW * ipad
     out = out or PT((opad, krow), planes, device=w.device)
     # rows = input channels (stride KH*KW), cols = output channels (stride I*KH*KW)

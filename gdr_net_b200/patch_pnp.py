@@ -2,8 +2,9 @@
 (core/gdrn_modeling/models/conv_pnp_net.py:111-157) on the sm_90a kernels -- BASELINE.json configs[3]
 ("64x64x(3+64) correspondence maps -> R|t, batch 512").
 
-    [B, 3|5, 64, 64] xyz (+2-D coords)  +  [B, 64, 64, 64] region attention  (+ extents [B, 3])
-        -> gdrn_pnp_pack_input   NCHW fp32 -> NHWC 16-bit planes, 67 | 69 valid of 128 channels, xyz de-normalised
+    [B, 3|5, 64, 64] xyz (+2-D coords)  +  [B, R, 64, 64] region attention, if any  (+ extents [B, 3])
+        -> gdrn_pnp_pack_input   NCHW fp32 -> NHWC 16-bit planes, nIn valid of round_up(nIn, 64) channels (64 or 128), xyz
+                                 de-normalised
         -> 3 x (wgmma implicit-GEMM conv 3x3 s2 -> GroupNorm(32)+ReLU)        64 -> 32 -> 16 -> 8
         -> fc1 (8192 -> 1024, LeakyReLU 0.1) -> fc2 (1024 -> 256, LeakyReLU) -> fc_r | fc_t (one 9-column GEMM)
         -> rot [B, 6], t [B, 3]  (fp32)
@@ -21,8 +22,8 @@ from .ops import PT, _stream
 
 
 def pnp_net_forward(x: PT, net, wf: dict, b_rt: torch.Tensor, pred: torch.Tensor, saved: list | None = None):
-    """3 x (conv 3x3 s2 -> GroupNorm + ReLU) -> fc1 -> fc2 -> fc_r|fc_t of `net` (a ConvPnPNet) on the 128-channel input
-    planes x [B, 64, 64, 128].  wf: packed operands "pnp_net.features.{0,3,6}" (pack_conv_fwd), "fc1", "fc2" and "fc_rt"
+    """3 x (conv 3x3 s2 -> GroupNorm + ReLU) -> fc1 -> fc2 -> fc_r|fc_t of `net` (a ConvPnPNet) on the input planes
+    x [B, 64, 64, round_up(nIn, 64)].  wf: packed operands "pnp_net.features.{0,3,6}" (pack_conv_fwd), "fc1", "fc2" and "fc_rt"
     (pack_linear of fc_r and fc_t stacked), b_rt their stacked bias.  pred [B, 16] fp32 receives rot in its first
     fc_r.out_features columns and t in the next 3.  saved: receives dict(ci, gi, x_in, u, y, gstats) per conv for backward.
     Returns the inputs of fc1, fc2 and fc_r|fc_t."""
@@ -51,6 +52,7 @@ class PatchPnP:
         self.net = pnp_net
         self.planes = 1 if precision == "half" else 2
         self.precision = precision
+        self.pnp_ld = -(-pnp_net.nIn // 64) * 64  # input row: 64 channels for nIn <= 64, else 128
         self.wf = {}
         self._wkey = None
         self._graphs = {}
@@ -66,7 +68,7 @@ class PatchPnP:
         dev = n.fc1.weight.device
         for ci in (0, 3, 6):
             k = f"pnp_net.features.{ci}"
-            wf[k] = ops.pack_conv_fwd(n.features[ci].weight.detach(), pl, out=wf.get(k), ipad=128)
+            wf[k] = ops.pack_conv_fwd(n.features[ci].weight.detach(), pl, out=wf.get(k), ipad=self.pnp_ld if ci == 0 else None)
         wf["fc1"] = ops.pack_linear(n.fc1.weight.detach(), pl, out=wf.get("fc1"), nhwc_from=(128, 8, 8))
         wf["fc2"] = ops.pack_linear(n.fc2.weight.detach(), pl, out=wf.get("fc2"))
         if "w_rt" not in wf:
@@ -83,9 +85,12 @@ class PatchPnP:
     def _run(self, coor_feat, region, extents, pred):
         B, c_feat = coor_feat.shape[0], coor_feat.shape[1]
         c_reg = 0 if region is None else region.shape[1]
-        x = PT((B, 64, 64, 128), self.planes, device=coor_feat.device)
-        C.gdrn_pnp_pack_input(coor_feat.data_ptr(), c_feat, ops.ptr(region), c_reg, ops.ptr(extents), x.hi_ptr, x.lo_ptr, B, 4096,
-                              _stream())
+        x = PT((B, 64, 64, self.pnp_ld), self.planes, device=coor_feat.device)
+        args = (coor_feat.data_ptr(), c_feat, ops.ptr(region), c_reg, ops.ptr(extents), x.hi_ptr, x.lo_ptr, B, 4096)
+        if self.pnp_ld == 128:
+            C.gdrn_pnp_pack_input(*args, _stream())
+        else:
+            C.gdrn_pnp_pack_input_ex(*args, self.pnp_ld, _stream())
         pnp_net_forward(x, self.net, self.wf, self.wf["b_rt"], pred)
 
     @torch.no_grad()

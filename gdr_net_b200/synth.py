@@ -74,8 +74,10 @@ def ycbv_like_symmetries() -> list:
     return _YCBV_SYMS
 
 
-def make_batch(bs: int, seed: int = 0, n_points: int = 3000, with_sym: bool = False, dtype=torch.float32) -> dict:
-    """Synthetic batch with the reference field names (CPU tensors)."""
+def make_batch(bs: int, seed: int = 0, n_points: int = 3000, with_sym: bool = False, dtype=torch.float32,
+               num_regions: int = 64) -> dict:
+    """Synthetic batch with the reference field names (CPU tensors); region labels 1..num_regions on the object, 0 off it
+    (ROT_HEAD.NUM_REGIONS; the default draws the same random stream as before the parameter existed)."""
     g = _gen(seed, "batch")
     H = W = 64
     roi_img = torch.rand(bs, 3, 256, 256, generator=g, dtype=dtype)
@@ -105,7 +107,7 @@ def make_batch(bs: int, seed: int = 0, n_points: int = 3000, with_sym: bool = Fa
     mask_trunc = mask_visib * (px < cut).float()
 
     roi_xyz = torch.rand(bs, 3, H, W, generator=g, dtype=dtype) * mask_obj[:, None]
-    roi_region = (torch.randint(1, 65, (bs, H, W), generator=g) * mask_obj.long()).long()
+    roi_region = (torch.randint(1, num_regions + 1, (bs, H, W), generator=g) * mask_obj.long()).long()
 
     roi_extent = 0.05 + 0.25 * torch.rand(bs, 3, generator=g, dtype=dtype)
     roi_points = (torch.rand(bs, n_points, 3, generator=g, dtype=dtype) - 0.5) * roi_extent[:, None, :]

@@ -168,6 +168,26 @@ int gdrn_head_bwd_ex(const float* logits, const float* gt_xyz, const float* m_xy
                      const long long* labels, const double* sums, const float* gw, const void* din_hi, const void* din_lo,
                      const float* extents, void* out_hi, void* out_lo, int B, int HW, int with_2d, int mask_loss, int mask_out,
                      void* stream);
+/* The same for any region count (ROT_HEAD.NUM_REGIONS = num_regions, 2..64) with or without region attention
+ * (PNP_NET.REGION_ATTENTION = region_att, 0 or 1).  A logit row is mask | xyz | bg | num_regions regions: N = mask_out + 4 +
+ * num_regions of 72 floats valid, the rest never read.  The Patch-PnP input is xyz | coord2d (with_2d) | softmax over the
+ * regions (region_att): nIn = 3 (+2) (+num_regions) channels in rows of pnp_ld = round_up(nIn, 64) = 64 or 128, the padding
+ * zeroed; head_bwd_ex2 reads d(Patch-PnP input) in that layout (only xyz / coord2d without attention) and zeroes gradient
+ * columns N .. 127.  The region CE runs over num_regions + 1 classes; a label above num_regions gives an unspecified loss.
+ * pixel_loss_fwd_ex2 checks region_att and pnp_ld but does not depend on them; head_bwd_ex2 with 64 regions and attention is
+ * head_bwd_ex.  gdrn_pnp_pack_input_ex is
+ * gdrn_pnp_pack_input into rows of pnp_ld = round_up(c_feat + c_reg, 64). */
+int gdrn_head_glue_fwd_ex2(const float* logits, const float* coord2d, const float* extents, void* out_hi, void* out_lo, int B,
+                           int HW, int with_2d, int mask_out, int num_regions, int region_att, int pnp_ld, void* stream);
+int gdrn_pixel_loss_fwd_ex2(const float* logits, const float* gt_xyz, const float* m_xyz, const float* m_mask,
+                            const float* m_region, const long long* labels, double* sums, int B, int HW, int mask_loss,
+                            int mask_out, int num_regions, int region_att, int pnp_ld, void* stream);
+int gdrn_head_bwd_ex2(const float* logits, const float* gt_xyz, const float* m_xyz, const float* m_mask, const float* m_region,
+                      const long long* labels, const double* sums, const float* gw, const void* din_hi, const void* din_lo,
+                      const float* extents, void* out_hi, void* out_lo, int B, int HW, int with_2d, int mask_loss, int mask_out,
+                      int num_regions, int region_att, int pnp_ld, void* stream);
+int gdrn_pnp_pack_input_ex(const float* coor_feat, int c_feat, const float* region, int c_reg, const float* extents,
+                           void* out_hi, void* out_lo, int B, int HW, int pnp_ld, void* stream);
 
 /* ---- rot6d -> R, SITE translation, allo -> ego, PM loss (+ closest symmetric GT), centroid / z losses, re/te
  * (rot_reps.py:34-49, pose_from_pred_centroid_z.py:144-227, utils.py:208-236, pm_loss.py:82-114,
