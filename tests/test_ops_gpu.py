@@ -1,6 +1,7 @@
 """GPU: every C-ABI op against a plain PyTorch fp32 reference of the same op (TF32 disabled).
-nsplit = 1 (bf16 operands): the reference is evaluated on bf16-rounded operands, so only fp32
-accumulation order differs.  nsplit = 3 (hi/lo planes): the reference is full fp32."""
+nsplit = 1 (one 16-bit plane, fp16 unless the library is built for bf16): the reference is evaluated on operands rounded to
+the storage format, so only fp32 accumulation order differs.  nsplit = 3 (hi/lo planes): the reference is full fp32.
+Per-launch float64 checks of the GEMM kernels at the engine's own shapes: tests/test_gemm_audit_gpu.py."""
 import math
 
 import pytest
