@@ -234,8 +234,10 @@ __global__ void __launch_bounds__(256, 4) bn_fwd_kernel(const bf16* __restrict__
     for (int c = threadIdx.x; c < C; c += blockDim.x) {
         float mean, var;
         if (train) {
-            const double m = (double)stats[c] / count;
-            double v = (double)stats[C + c] / count - m * m;
+            // train & 2: the statistics were accumulated in double (GEMM epilogue with kActStatsF64)
+            const double* s64 = reinterpret_cast<const double*>(stats);
+            const double m = ((train & 2) ? s64[c] : (double)stats[c]) / count;
+            double v = ((train & 2) ? s64[C + c] : (double)stats[C + c]) / count - m * m;
             if (v < 0) v = 0;
             mean = (float)m;
             var = (float)v;

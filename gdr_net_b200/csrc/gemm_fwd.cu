@@ -261,8 +261,13 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_fwd_kernel(const __grid_cons
         for (int i = threadIdx.x; i < BLOCK_N; i += 256) {
             const int col = n_tile * BLOCK_N + i;
             if (col < p.N) {
-                atomicAdd(p.stats + col, s_stats[i]);
-                atomicAdd(p.stats + p.N + col, s_stats[BLOCK_N + i]);
+                if (p.stats_f64) {
+                    atomicAdd(reinterpret_cast<double*>(p.stats) + col, (double)s_stats[i]);
+                    atomicAdd(reinterpret_cast<double*>(p.stats) + p.N + col, (double)s_stats[BLOCK_N + i]);
+                } else {
+                    atomicAdd(p.stats + col, s_stats[i]);
+                    atomicAdd(p.stats + p.N + col, s_stats[BLOCK_N + i]);
+                }
             }
         }
     }
@@ -344,7 +349,7 @@ extern "C" int gdrn_conv_fwd(const void* x_hi, const void* x_lo, const void* w_h
     if (ldc % 8 != 0 || ldc < Cout) return set_error(GDRN_ERR_ARG, "conv_fwd: bad ldc=%d", ldc);
     if (res_hi != nullptr && (Cout % 32 != 0 || y_hi == nullptr))
         return set_error(GDRN_ERR_ARG, "conv_fwd: a residual needs Cout %% 32 == 0 and a 16-bit output");
-    if (act < 0 || act > 2) return set_error(GDRN_ERR_ARG, "conv_fwd: act must be 0 (none), 1 (LeakyReLU 0.1) or 2 (ReLU)");
+    if ((act & ~kActStatsF64) < 0 || (act & ~kActStatsF64) > 2) return set_error(GDRN_ERR_ARG, "conv_fwd: act must be 0 (none), 1 (LeakyReLU 0.1) or 2 (ReLU)");
     const int Ho = H / stride, Wo = W / stride;
     if (Wo > 128 || 128 % Wo != 0) return set_error(GDRN_ERR_ARG, "conv_fwd: unsupported output width %d", Wo);
     if ((uint64_t)N * Ho * Wo * ldc > UINT32_MAX) return set_error(GDRN_ERR_ARG, "conv_fwd: output too large for 32-bit offsets");
@@ -396,8 +401,9 @@ extern "C" int gdrn_conv_fwd(const void* x_hi, const void* x_lo, const void* w_h
     p.bias = bias;
     p.res_hi = res_hi;
     p.res_lo = res_lo;
-    p.act = act;
+    p.act = act & ~kActStatsF64;
     p.stats = stats;
+    p.stats_f64 = (act & kActStatsF64) ? 1 : 0;
     return dispatch_gemm(p, block_n, nsplit, stream);
 }
 
@@ -459,8 +465,9 @@ extern "C" int gdrn_conv_dgrad_s2(const void* du_hi, const void* du_lo, const vo
     p.out_lo = dx_lo;
     p.ldc = ldc;
     p.bias = bias;    // the same kernel is the FORWARD of ConvTranspose2d(k3, s2, p1, op1) (cdpn_rot_head_region.py:82-91): then
-    p.act = act;      // bias / activation (folded eval BatchNorm) and the BatchNorm batch statistics apply to its output
+    p.act = act & ~kActStatsF64;  // bias / activation (folded eval BatchNorm) and the BatchNorm batch statistics apply to its output
     p.stats = stats;
+    p.stats_f64 = (act & kActStatsF64) ? 1 : 0;
     // phases in order of decreasing tap count (longest tiles first on the persistent CTAs)
     p.nphase = nphase;
     int nt = 0;
@@ -524,8 +531,9 @@ extern "C" int gdrn_gemm_fwd(const void* a_hi, const void* a_lo, const void* w_h
     p.out_f32 = y_f32;
     p.ldc = ldc;
     p.bias = bias;
-    p.act = act;
+    p.act = act & ~kActStatsF64;
     p.stats = stats;
+    p.stats_f64 = (act & kActStatsF64) ? 1 : 0;
     return dispatch_gemm(p, block_n, nsplit, stream);
 }
 

@@ -4,6 +4,9 @@
 
 namespace gdrn {
 
+// flag bit of the `act` argument of gdrn_conv_fwd / gdrn_gemm_fwd / gdrn_conv_dgrad_s2: `stats` is double [2][N]
+constexpr int kActStatsF64 = 16;
+
 struct GemmParams {
     CUtensorMap tmA[2][4];  // [plane hi/lo][stride-2 phase]
     CUtensorMap tmB[2];     // [plane hi/lo]
@@ -21,6 +24,8 @@ struct GemmParams {
     const void* res_lo;  // the eval-mode folded conv + BN + (identity) + ReLU epilogue of a BasicBlock's second conv
     int act;       // 0 none, 1 LeakyReLU(0.1), 2 ReLU
     float* stats;  // [2][N]: sum, sum of squares (accumulated with atomics) or nullptr
+    int stats_f64; // stats points to double [2][N] (the act argument's GDRN_ACT_STATS_F64 bit): the CTAs' partial sums are added
+                   // in double, so the result no longer depends on the order of the atomics beyond fp32 rounding of each partial
     // Stride-2 dgrad by output-parity phases (mode 1, nphase > 0): rows index the (n, i, j) lattice of dY; phase ph writes
     // output pixel (2i + ph_a, 2j + ph_b) and sums taps [ph_tap0[ph], ph_tap0[ph+1]) of the tables below
     // (dY offset (tap_dh, tap_dw); tap_w = tap slot of the packed weight matrix).  Tiles are enumerated phase-major.

@@ -103,6 +103,7 @@ class _BN:
         self.invstd = torch.empty(C_, device=dev)
         self.sums = torch.empty(2, C_, device=dev)
         self.stats = None  # view into Engine.stats_all
+        self.stats64 = None  # view into Engine.stats64_all: the epilogue statistics of the atomic path
 
 
 class SymTable:
@@ -215,11 +216,15 @@ class Engine:
                 self._bn_mods[name] = m
                 total += 2 * m.num_features
         self.stats_all = torch.zeros(total, device=self.dev)
+        # GEMM-epilogue statistics (deterministic = False): the CTAs' partial sums are added in double, so the result does not
+        # move with the order of the atomics beyond the fp32 rounding of each partial
+        self.stats64_all = torch.zeros(total, dtype=torch.float64, device=self.dev)
         self.bwd_sums_all = torch.zeros(total, device=self.dev)  # BN-backward accumulators: one memset per backward
         off = 0
         for name, m in self._bn_mods.items():
             n = 2 * m.num_features
             self.bn[name].stats = self.stats_all[off:off + n]
+            self.bn[name].stats64 = self.stats64_all[off:off + n]
             self.bn[name].sums = self.bwd_sums_all[off:off + n].view(2, m.num_features)
             off += n
         # flat gradient buffer (one NCCL-friendly allocation); per-parameter views
@@ -505,9 +510,10 @@ class Engine:
             mask = torch.empty(u.numel() // 8, dtype=torch.uint8, device=self.dev)
         self._last_mask = mask
         C.gdrn_bn_fwd(u.hi_ptr, u.lo_ptr, res.hi_ptr if res else None, res.lo_ptr if res else None, y.hi_ptr, y.lo_ptr,
-                      ops.ptr(st.stats) if train_bn else None, mod.weight.data_ptr(), mod.bias.data_ptr(),
-                      mod.running_mean.data_ptr(), mod.running_var.data_ptr(), st.mean.data_ptr(), st.invstd.data_ptr(),
-                      ops.ptr(mask), count, Cc, float(mod.eps), float(mom), int(train_bn), int(relu), _stream())
+                      ops.ptr(st.stats if self.deterministic else st.stats64) if train_bn else None, mod.weight.data_ptr(),
+                      mod.bias.data_ptr(), mod.running_mean.data_ptr(), mod.running_var.data_ptr(), st.mean.data_ptr(),
+                      st.invstd.data_ptr(), ops.ptr(mask), count, Cc, float(mod.eps), float(mom),
+                      int(train_bn) | (2 if train_bn and not self.deterministic else 0), int(relu), _stream())
         return y
 
     def _det_workspace(self):
@@ -516,7 +522,7 @@ class Engine:
         return self._det_ws
 
     def _conv_bn(self, x: PT, ckey: str, conv, bkey: str, relu: bool, train_bn: bool, res: Optional[PT] = None):
-        stats = self.bn[bkey].stats if (train_bn and not self.deterministic) else None  # deterministic: from gdrn_bn_stats
+        stats = self.bn[bkey].stats64 if (train_bn and not self.deterministic) else None  # deterministic: from gdrn_bn_stats
         k, stride, pad = conv.kernel_size[0], conv.stride[0], conv.padding[0]
         if ckey == "deconv":
             u = ops.conv_dgrad_s2(x, self.wf["deconv"], conv.out_channels, 3, 1, stats=stats)
@@ -579,7 +585,7 @@ class Engine:
         self._on_side(lambda: self.prepare_weights(need_dgrad=do_loss))
         self._nbt = []
         if train_bn:
-            self.stats_all.zero_()
+            (self.stats_all if self.deterministic else self.stats64_all).zero_()
         S = dict(B=B, train_bn=train_bn) if do_loss else None
         self._want_masks = do_loss
 
@@ -588,7 +594,7 @@ class Engine:
         C.gdrn_stem_im2col(x.data_ptr(), a_col.hi_ptr, a_col.lo_ptr, B, 256, 256, _stream())
         self._join_side(force=True)
         st0 = self.bn["backbone.bn1"]
-        u0 = ops.gemm_fwd(a_col, self.wf["stem"], 64, stats=st0.stats if (train_bn and not self.deterministic) else None).view(B, 128, 128, 64)
+        u0 = ops.gemm_fwd(a_col, self.wf["stem"], 64, stats=st0.stats64 if (train_bn and not self.deterministic) else None).view(B, 128, 128, 64)
         a0 = self._bn_fwd("backbone.bn1", u0, True, train_bn)
         if S is not None:
             cur, pool_arg = ops.maxpool_fwd(a0, want_arg=True)

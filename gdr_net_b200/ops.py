@@ -104,6 +104,14 @@ class PT:
         return y
 
 
+ACT_STATS_F64 = 16  # act flag bit of the GEMM entry points: the epilogue statistics buffer is double (include/gdrn_b200.h)
+
+
+def _act(act: int, stats) -> int:
+    """act with ACT_STATS_F64 set when the statistics buffer is float64."""
+    return act | ACT_STATS_F64 if stats is not None and stats.dtype == torch.float64 else act
+
+
 def _round_up(x, m):
     return (x + m - 1) // m * m
 
@@ -220,7 +228,7 @@ def conv_fwd(x: PT, wp: PT, Cout: int, KH: int, KW: int, stride: int, pad: int, 
     C.gdrn_conv_fwd(x.hi_ptr, x.lo_ptr, wp.hi_ptr, wp.lo_ptr, out.hi_ptr if out is not None else None,
                     out.lo_ptr if out is not None else None, ptr(out_f32), ptr(bias), res.hi_ptr if res is not None else None,
                     res.lo_ptr if res is not None else None, ptr(stats), N, H, W, Cin, Cout, wp.shape[0], KH, KW, stride, pad,
-                    ldc, act, x.nsplit, _stream())
+                    ldc, _act(act, stats), x.nsplit, _stream())
     return out
 
 
@@ -232,7 +240,7 @@ def conv_dgrad_s2(du: PT, wd: PT, Cx: int, K: int, pad: int, *, out: PT | None =
     if out is None:
         out = PT((N, 2 * Ho, 2 * Wo, ldc), du.planes, device=du.buf.device, zero=(K == 1 or ldc != Cx))
     C.gdrn_conv_dgrad_s2(du.hi_ptr, du.lo_ptr, wd.hi_ptr, wd.lo_ptr, out.hi_ptr, out.lo_ptr, ptr(bias), ptr(stats), N, Ho, Wo, Cy, Cx,
-                         wd.shape[0], K, pad, ldc, act, du.nsplit, _stream())
+                         wd.shape[0], K, pad, ldc, _act(act, stats), du.nsplit, _stream())
     return out
 
 
@@ -244,7 +252,7 @@ def gemm_fwd(a: PT, wp: PT, N: int, *, out: PT | None = None, out_f32: torch.Ten
         out = PT((M, ldc), a.planes, device=a.buf.device, zero=(ldc != N))
     C.gdrn_gemm_fwd(a.hi_ptr, a.lo_ptr, wp.hi_ptr, wp.lo_ptr, out.hi_ptr if out is not None else None,
                     out.lo_ptr if out is not None else None, ptr(out_f32), ptr(bias), ptr(stats), M, N, wp.shape[0], K, ldc,
-                    act, a.nsplit, _stream())
+                    _act(act, stats), a.nsplit, _stream())
     return out
 
 

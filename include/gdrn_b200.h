@@ -42,7 +42,9 @@ int gdrn_last_gemm_variant(void); /* BLOCK_N*10 + nsplit of this thread's last c
  * weights (gdrn_bn_fold_batched + row_scale of the pack jobs) and bias = the folded shift this is the eval-mode fused
  * conv + BN (+ identity) + ReLU of resnet_backbone.py:69-76 / torchvision BasicBlock / cdpn_rot_head_region.py:82-125.
  * stats (optional) [2][Cout] fp32 += per-channel sum and sum of squares of the fp32 accumulators
- * (BatchNorm batch statistics, reference get_norm("BN") layers). */
+ * (BatchNorm batch statistics, reference get_norm("BN") layers).  With GDRN_ACT_STATS_F64 set in act, stats is double [2][Cout]
+ * and each CTA's fp32 partial sums are added in double (the same applies to gdrn_gemm_fwd and gdrn_conv_dgrad_s2). */
+#define GDRN_ACT_STATS_F64 16
 int gdrn_conv_fwd(const void* x_hi, const void* x_lo, const void* w_hi, const void* w_lo, void* y_hi, void* y_lo,
                   float* y_f32, const float* bias, const void* res_hi, const void* res_lo, float* stats, int N, int H, int W,
                   int Cin, int Cout, int Cout_pad, int KH, int KW, int stride, int pad, int ldc, int act, int nsplit,
@@ -94,7 +96,8 @@ int gdrn_bn_finalize(const float* stats, const float* gamma, const float* beta, 
                      float momentum, int train, void* stream);
 /* finalize + apply in one kernel (what the engine uses): batch statistics from the conv epilogue -> y, running stats.
  * relu_mask_out (optional, with relu): uint8 [rows*C/8], bit j of byte i = [pre-activation of element 8i+j > 0]; BatchNorm
- * backward (relu_mask) reads it instead of the activation to rebuild the ReLU mask (1/8 B instead of 2 B per element). */
+ * backward (relu_mask) reads it instead of the activation to rebuild the ReLU mask (1/8 B instead of 2 B per element).
+ * train = 3: stats is double [2][C] (a GEMM epilogue with GDRN_ACT_STATS_F64). */
 int gdrn_bn_fwd(const void* x_hi, const void* x_lo, const void* r_hi, const void* r_lo, void* y_hi, void* y_lo,
                 const float* stats, const float* gamma, const float* beta, float* running_mean, float* running_var,
                 float* mean_out, float* invstd_out, void* relu_mask_out, long rows, int C, float eps, float momentum, int train,

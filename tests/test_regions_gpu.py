@@ -114,7 +114,7 @@ def test_b64_mixed_matches_oracle(case):
         ref = float(o["losses"][k])
         print(f"[{case}] B=64 {k}: {v:.6f} vs {ref:.6f} rel {abs(v - ref) / abs(ref):.2e}")
         assert abs(v - ref) <= REL * abs(ref), (k, v, ref)
-    assert all(torch.isfinite(p.grad).all() for n, p in model.named_parameters() if n != "backbone.conv1.weight")
+    assert all(torch.isfinite(p.grad).all() for p in model.parameters())
 
 
 @pytest.mark.parametrize("case", ["r8", "r32_noatt", "r60"])
@@ -206,5 +206,5 @@ def test_roi_targets_with_8_anchors_feed_an_8_region_train_step():
     print("chained r8 losses", ld)
     assert all(math.isfinite(v) for v in ld.values())
     assert ld["loss_region"] > 0
-    assert all(torch.isfinite(p.grad).all() for n, p in model.named_parameters() if n != "backbone.conv1.weight")
+    assert all(torch.isfinite(p.grad).all() for p in model.parameters())
     assert np.isfinite(model.rot_head_net.features[23].weight.grad.cpu().numpy()).all()
