@@ -18,7 +18,7 @@ from typing import Optional
 import torch
 import torch.nn as nn
 
-from .engine import Engine, LOSS_NAMES, pose_loss_switches  # noqa: F401  (LOSS_NAMES: the default list, re-exported)
+from .engine import Engine, LOSS_NAMES, check_roi_classes, pose_loss_switches  # noqa: F401  (LOSS_NAMES: the default list, re-exported)
 
 logger = logging.getLogger(__name__)
 
@@ -90,10 +90,12 @@ class ResNetBackboneNet(_ParamsOnly):
 
 class RotWithRegionHead(_ParamsOnly):
     """reference models/cdpn_rot_head_region.py:10-143 (ROT_CONCAT=False branch; concat mode is broken
-    upstream, SURVEY P8).  `features` keeps the reference indices: ReLU / upsample placeholders included."""
+    upstream, SURVEY P8).  `features` keeps the reference indices: ReLU / upsample placeholders included.
+    With rot / mask / region_class_aware the output conv carries that block once per class (engine.class_rows)."""
 
     def __init__(self, in_channels=512, num_layers=3, num_filters=256, kernel_size=3, output_kernel_size=1,
-                 rot_output_dim=3, mask_output_dim=1, num_regions=64, norm="BN", freeze=False):
+                 rot_output_dim=3, mask_output_dim=1, num_regions=64, norm="BN", freeze=False, num_classes=1,
+                 rot_class_aware=False, mask_class_aware=False, region_class_aware=False):
         super().__init__()
         if kernel_size != 3 or output_kernel_size != 1 or norm != "BN" or num_layers != 3:
             raise NotImplementedError("only the a6 head (k3 deconv, 1x1 output conv, BN, 3 stages) is implemented")
@@ -109,10 +111,10 @@ class RotWithRegionHead(_ParamsOnly):
                 f.append(nn.Conv2d(num_filters, num_filters, 3, 1, 1, bias=False))
                 f.append(nn.BatchNorm2d(num_filters))
                 f.append(nn.ReLU(inplace=True))
-        self.rot_output_dim = rot_output_dim
-        self.mask_output_dim = mask_output_dim
-        self.region_output_dim = num_regions + 1
-        f.append(nn.Conv2d(num_filters, mask_output_dim + rot_output_dim + self.region_output_dim, 1, padding=0, bias=True))
+        self.rot_output_dim = rot_output_dim * (num_classes if rot_class_aware else 1)
+        self.mask_output_dim = mask_output_dim * (num_classes if mask_class_aware else 1)
+        self.region_output_dim = (num_regions + 1) * (num_classes if region_class_aware else 1)
+        f.append(nn.Conv2d(num_filters, self.mask_output_dim + self.rot_output_dim + self.region_output_dim, 1, padding=0, bias=True))
         self.features = f
         for m in self.modules():
             if isinstance(m, (nn.Conv2d, nn.ConvTranspose2d)):
@@ -193,8 +195,10 @@ def _check_supported(cfg):
     problems = []
     if c.BACKBONE.NUM_LAYERS not in resnet_spec or c.BACKBONE.INPUT_RES != 256 or c.BACKBONE.OUTPUT_RES != 64:
         problems.append("backbone must be resnet18/34 at 256 -> 64")
-    if r.ROT_CONCAT or r.ROT_CLASS_AWARE or r.MASK_CLASS_AWARE or r.REGION_CLASS_AWARE:
-        problems.append("class-aware / concat heads")
+    if r.ROT_CONCAT:
+        problems.append("concat heads (ROT_HEAD.ROT_CONCAT)")
+    if (r.ROT_CLASS_AWARE or r.MASK_CLASS_AWARE or r.REGION_CLASS_AWARE) and not int(r.NUM_CLASSES) >= 1:
+        problems.append(f"ROT_HEAD.NUM_CLASSES = {r.NUM_CLASSES!r} with a class-aware head (>= 1)")
     if r.XYZ_LOSS_TYPE != "L1" or r.MASK_LOSS_TYPE not in ("L1", "BCE", "CE") or r.REGION_LOSS_TYPE != "CE":
         problems.append("losses other than xyz L1 / mask L1, BCE or CE / region CE")
     # the per-pixel kernels hold a logit row of 72 floats: MO + 3 + (R + 1) <= 70 for R <= 64; R < 2 fails the reference's own
@@ -270,25 +274,28 @@ class GDRN(nn.Module):
                 gt_points=None, sym_infos=None, gt_trans=None, gt_trans_ratio=None, roi_classes=None, roi_coord_2d=None,
                 roi_cams=None, roi_centers=None, roi_whs=None, roi_extents=None, resize_ratios=None, do_loss=False):
         cfg = self.cfg
+        r_cfg = cfg.MODEL.CDPN.ROT_HEAD
+        if r_cfg.ROT_CLASS_AWARE or r_cfg.MASK_CLASS_AWARE or r_cfg.REGION_CLASS_AWARE:
+            check_roi_classes(roi_classes, x.shape[0], int(r_cfg.NUM_CLASSES))
         if not x.is_cuda:
             raise RuntimeError("gdr_net_b200.GDRN runs on CUDA (sm_90a) only; there is no CPU fallback")
         pnp_cfg = cfg.MODEL.CDPN.PNP_NET
         res = self.engine.run(
-            x, roi_coord_2d=roi_coord_2d, roi_cams=roi_cams, roi_centers=roi_centers, roi_whs=roi_whs,
-            roi_extents=roi_extents, resize_ratios=resize_ratios, gt_xyz=gt_xyz, gt_mask_trunc=gt_mask_trunc,
+            x, roi_classes=roi_classes, roi_coord_2d=roi_coord_2d, roi_cams=roi_cams, roi_centers=roi_centers,
+            roi_whs=roi_whs, roi_extents=roi_extents, resize_ratios=resize_ratios, gt_xyz=gt_xyz, gt_mask_trunc=gt_mask_trunc,
             gt_mask_visib=gt_mask_visib, gt_mask_obj=gt_mask_obj, gt_region=gt_region, gt_ego_rot=gt_ego_rot, gt_points=gt_points,
             sym_infos=sym_infos if pnp_cfg.PM_LOSS_SYM else None, gt_trans=gt_trans, gt_trans_ratio=gt_trans_ratio,
             do_loss=do_loss, train_bn=self.training, want_maps=(not do_loss) and bool(cfg.TEST.USE_PNP),
         )
         if not do_loss:
             # NOTE: the reference returns `rot` on the CPU in test mode (numpy loop, pose_from_pred_centroid_z.py:141);
-            # we keep it on the device -- `.cpu()` is a no-op for consumers that need host data.
+            # we keep it on the device -- `.cpu()` is a no-op for consumers that need host data.  With a class-aware head the
+            # maps are those of each crop's class (GDRN.py:134-151).
             out_dict = {"rot": res["rot"], "trans": res["trans"]}
             if cfg.TEST.USE_PNP:
                 out_dict.update({k: res[k] for k in ("mask", "coor_x", "coor_y", "coor_z", "region")})
             return out_dict
         assert (gt_xyz is not None) and (gt_trans is not None) and (gt_trans_ratio is not None) and (gt_region is not None)
-        r_cfg = cfg.MODEL.CDPN.ROT_HEAD
         lw = dict(loss_coor_x=r_cfg.XYZ_LW, loss_coor_y=r_cfg.XYZ_LW, loss_coor_z=r_cfg.XYZ_LW, loss_mask=r_cfg.MASK_LW,
                   loss_region=r_cfg.REGION_LW, loss_rot=pnp_cfg.ROT_LW, loss_centroid=pnp_cfg.CENTROID_LW, loss_z=pnp_cfg.Z_LW,
                   loss_trans_xy=pnp_cfg.TRANS_LW, loss_trans_z=pnp_cfg.TRANS_LW, loss_trans_LPnP=pnp_cfg.TRANS_LW,
@@ -368,6 +375,8 @@ def build_model_optimizer(cfg, precision: str = "mixed"):
         channels[-1], r_head_cfg.NUM_LAYERS, r_head_cfg.NUM_FILTERS, r_head_cfg.CONV_KERNEL_SIZE,
         r_head_cfg.OUT_CONV_KERNEL_SIZE, rot_output_dim=r_out_dim, mask_output_dim=mask_out_dim,
         num_regions=r_head_cfg.NUM_REGIONS, norm=r_head_cfg.NORM, freeze=r_head_cfg.FREEZE,
+        num_classes=r_head_cfg.NUM_CLASSES, rot_class_aware=r_head_cfg.ROT_CLASS_AWARE,
+        mask_class_aware=r_head_cfg.MASK_CLASS_AWARE, region_class_aware=r_head_cfg.REGION_CLASS_AWARE,
     )
     params_lr_list.append({"params": [p for p in rot_head_net.parameters() if p.requires_grad], "lr": float(cfg.SOLVER.BASE_LR)})
 

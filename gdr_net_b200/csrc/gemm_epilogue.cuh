@@ -17,9 +17,10 @@ namespace gdrn {
 // shared by the output and residual planes; the host entry points reject outputs with rows * ldc >= 2^32.  Addresses are
 // rebuilt from the kernel parameters for every chunk: unsigned arithmetic keeps the compiler from hoisting them into 64-bit
 // per-row pointers, which would not fit next to the accumulators of a 128-wide 3-pass tile.
-template <int BLOCK_N>
+// GROUPED: the bias of this tile starts at p.bias + bias_off (the tile's weight group, gemm_fwd_grouped_kernel).
+template <int BLOCK_N, bool GROUPED = false>
 __device__ __forceinline__ void gemm_epilogue_tile(const GemmParams& p, const float* acc, int lane, int row0, int m_tile, int n_tile,
-                                                   int ph, float* s_stats) {
+                                                   int ph, float* s_stats, int bias_off = 0) {
     __nv_bfloat16* out_hi = reinterpret_cast<__nv_bfloat16*>(p.out_hi);
     __nv_bfloat16* out_lo = reinterpret_cast<__nv_bfloat16*>(p.out_lo);
     const __nv_bfloat16* res_hi = reinterpret_cast<const __nv_bfloat16*>(p.res_hi);
@@ -53,7 +54,9 @@ __device__ __forceinline__ void gemm_epilogue_tile(const GemmParams& p, const fl
 #pragma unroll
             for (int e = 0; e < 2; ++e) f[h][e] = acc[4 * j + 2 * h + e];
         if (p.bias != nullptr) {
-            const float b0 = ok0 ? __ldg(p.bias + col) : 0.f, b1 = ok1 ? __ldg(p.bias + col + 1) : 0.f;
+            // (the group offset is spelled inside each load: a hoisted bias pointer costs the ungrouped kernels registers)
+            const int c0 = GROUPED ? bias_off + col : col;
+            const float b0 = ok0 ? __ldg(p.bias + c0) : 0.f, b1 = ok1 ? __ldg(p.bias + c0 + 1) : 0.f;
 #pragma unroll
             for (int h = 0; h < 2; ++h) {
                 f[h][0] += b0;

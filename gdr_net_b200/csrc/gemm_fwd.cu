@@ -60,8 +60,15 @@ struct GemmCfg {
     static_assert(STAGES >= 2, "pipeline too shallow");
 };
 
-template <int BLOCK_N, int NSPLIT>
-__global__ void __launch_bounds__(kThreads, 1) gemm_fwd_kernel(const __grid_constant__ GemmParams p) {
+// Weight group of an M-tile (GROUPED): tiles never straddle a group (the entry points require rows_per_group % 128 == 0), and
+// the group id read from device memory is clamped so that neither the weight tile nor the bias is read outside the tables.
+__device__ __forceinline__ int tile_group(const GemmParams& p, int m_tile) {
+    const int g = __ldg(p.group + (m_tile * kBlockM) / p.rows_per_group);
+    return min(max(g, 0), p.num_w_groups - 1);
+}
+
+template <int BLOCK_N, int NSPLIT, bool GROUPED>
+__device__ __forceinline__ void gemm_fwd_body(const GemmParams& p) {
     using Cfg = GemmCfg<BLOCK_N, NSPLIT>;
     constexpr int NPL = Cfg::NPL;
     constexpr int STAGES = Cfg::STAGES;
@@ -119,7 +126,7 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_fwd_kernel(const __grid_cons
             }
             const int n_tile = rem % p.num_n_tiles;
             const int m_tile = rem / p.num_n_tiles;
-            const int bn0 = n_tile * BLOCK_N;
+            const int bn0 = n_tile * BLOCK_N + (GROUPED ? tile_group(p, m_tile) * p.w_group_rows : 0);
             if (mode == 1) {
                 int n0 = 0, h0 = 0;
                 if (p.TN == 1) {
@@ -253,7 +260,12 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_fwd_kernel(const __grid_cons
                 asm volatile("" : "+f"(acc[i]));
             }
         }
-        gemm_epilogue_tile<BLOCK_N>(p, acc, lane, cw * 64 + (warp & 3) * 16 + (lane >> 2), m_tile, n_tile, ph, s_stats);
+        if constexpr (GROUPED) {
+            gemm_epilogue_tile<BLOCK_N, true>(p, acc, lane, cw * 64 + (warp & 3) * 16 + (lane >> 2), m_tile, n_tile, ph, s_stats,
+                                              tile_group(p, m_tile) * p.bias_stride);
+        } else {
+            gemm_epilogue_tile<BLOCK_N>(p, acc, lane, cw * 64 + (warp & 3) * 16 + (lane >> 2), m_tile, n_tile, ph, s_stats);
+        }
     }
     if (p.stats != nullptr) {
         asm volatile("bar.sync 1, 256;" ::: "memory");  // the two MMA warpgroups only
@@ -273,13 +285,24 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_fwd_kernel(const __grid_cons
     }
 }
 
+template <int BLOCK_N, int NSPLIT>
+__global__ void __launch_bounds__(kThreads, 1) gemm_fwd_kernel(const __grid_constant__ GemmParams p) {
+    gemm_fwd_body<BLOCK_N, NSPLIT, false>(p);
+}
+
+// Per-group weights: the class-aware 1x1 output conv and its dgrad, where every crop (4096 rows) reads its class's weight rows.
+template <int BLOCK_N, int NSPLIT>
+__global__ void __launch_bounds__(kThreads, 1) gemm_fwd_grouped_kernel(const __grid_constant__ GemmParams p) {
+    gemm_fwd_body<BLOCK_N, NSPLIT, true>(p);
+}
+
 // ------------------------------------------------------------------------------------------------
 // host side
 // ------------------------------------------------------------------------------------------------
-template <int BLOCK_N, int NSPLIT>
+template <int BLOCK_N, int NSPLIT, bool GROUPED>
 static int launch_gemm(const GemmParams& p, cudaStream_t stream) {
     using Cfg = GemmCfg<BLOCK_N, NSPLIT>;
-    auto kern = gemm_fwd_kernel<BLOCK_N, NSPLIT>;
+    auto kern = GROUPED ? gemm_fwd_grouped_kernel<BLOCK_N, NSPLIT> : gemm_fwd_kernel<BLOCK_N, NSPLIT>;
     static bool attr_set = false;
     if (!attr_set) {
         GDRN_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
@@ -311,16 +334,33 @@ static int launch_gemm(const GemmParams& p, cudaStream_t stream) {
 
 static thread_local int g_last_variant = 0;
 
+template <bool GROUPED>
 static int dispatch_gemm(const GemmParams& p, int block_n, int nsplit, cudaStream_t stream) {
     g_last_variant = block_n * 10 + nsplit;
     if (nsplit == 1) {
-        if (block_n == 128) return launch_gemm<128, 1>(p, stream);
-        if (block_n == 64) return launch_gemm<64, 1>(p, stream);
+        if (block_n == 128) return launch_gemm<128, 1, GROUPED>(p, stream);
+        if (block_n == 64) return launch_gemm<64, 1, GROUPED>(p, stream);
     } else if (nsplit == 3) {
-        if (block_n == 128) return launch_gemm<128, 3>(p, stream);
-        if (block_n == 64) return launch_gemm<64, 3>(p, stream);
+        if (block_n == 128) return launch_gemm<128, 3, GROUPED>(p, stream);
+        if (block_n == 64) return launch_gemm<64, 3, GROUPED>(p, stream);
     }
     return set_error(GDRN_ERR_ARG, "gemm: unsupported block_n=%d nsplit=%d", block_n, nsplit);
+}
+
+static int dispatch_gemm(const GemmParams& p, int block_n, int nsplit, cudaStream_t stream) {
+    return p.group != nullptr ? dispatch_gemm<true>(p, block_n, nsplit, stream) : dispatch_gemm<false>(p, block_n, nsplit, stream);
+}
+
+// Grouped weights (gdrn_conv_fwd_grouped / gdrn_gemm_fwd_grouped): the argument checks shared by both, without touching the device.
+static int check_groups(const char* fn, const int* group, int M, int rows_per_group, int num_groups, int bias_stride, bool has_bias) {
+    if (group == nullptr) return set_error(GDRN_ERR_ARG, "%s: group is NULL", fn);
+    if (num_groups < 1) return set_error(GDRN_ERR_ARG, "%s: num_groups=%d must be >= 1", fn, num_groups);
+    if (rows_per_group <= 0 || rows_per_group % kBlockM != 0)
+        return set_error(GDRN_ERR_ARG, "%s: rows_per_group=%d must be a positive multiple of %d (tiles never straddle a group)", fn,
+                         rows_per_group, kBlockM);
+    if (M % rows_per_group != 0) return set_error(GDRN_ERR_ARG, "%s: M=%d is not a whole number of groups of %d rows", fn, M, rows_per_group);
+    if (has_bias && bias_stride < 0) return set_error(GDRN_ERR_ARG, "%s: bias_stride=%d must be >= 0", fn, bias_stride);
+    return 0;
 }
 
 // Tile width: the widest BLOCK_N (fewest A re-reads, best smem-bandwidth ratio) that still yields >= ~0.75 waves of
@@ -336,10 +376,10 @@ static int pick_block_n(int n_pad, int num_m_tiles) {
 
 using namespace gdrn;
 
-extern "C" int gdrn_conv_fwd(const void* x_hi, const void* x_lo, const void* w_hi, const void* w_lo, void* y_hi,
-                             void* y_lo, float* y_f32, const float* bias, const void* res_hi, const void* res_lo, float* stats,
-                             int N, int H, int W, int Cin, int Cout, int Cout_pad, int KH, int KW, int stride, int pad, int ldc,
-                             int act, int nsplit, void* stream_) {
+static int conv_fwd_impl(const void* x_hi, const void* x_lo, const void* w_hi, const void* w_lo, void* y_hi, void* y_lo,
+                         float* y_f32, const float* bias, const void* res_hi, const void* res_lo, float* stats, int N, int H, int W,
+                         int Cin, int Cout, int Cout_pad, int KH, int KW, int stride, int pad, int ldc, int act, int nsplit,
+                         const int* group, int rows_per_group, int num_groups, int bias_stride, void* stream_) {
     cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
     if (nsplit != 1 && nsplit != 3) return set_error(GDRN_ERR_ARG, "conv_fwd: nsplit must be 1 or 3");
     if (nsplit == 3 && (x_lo == nullptr || w_lo == nullptr)) return set_error(GDRN_ERR_ARG, "conv_fwd: lo planes missing");
@@ -376,7 +416,7 @@ extern "C" int gdrn_conv_fwd(const void* x_hi, const void* x_lo, const void* w_h
             const void* base = xb + ((size_t)phh * W + phw) * Cin;
             if (make_tmap(&p.tmA[pl][ph], base, 4, dims, strides, box)) return GDRN_ERR_CUDA;
         }
-        uint64_t wdims[2] = {(uint64_t)K, (uint64_t)Cout_pad};
+        uint64_t wdims[2] = {(uint64_t)K, (uint64_t)Cout_pad * num_groups};
         uint64_t wstr[1] = {(uint64_t)K * 2};
         uint32_t wbox[2] = {64, (uint32_t)block_n};
         if (make_tmap(&p.tmB[pl], ws[pl], 2, wdims, wstr, wbox)) return GDRN_ERR_CUDA;
@@ -404,7 +444,34 @@ extern "C" int gdrn_conv_fwd(const void* x_hi, const void* x_lo, const void* w_h
     p.act = act & ~kActStatsF64;
     p.stats = stats;
     p.stats_f64 = (act & kActStatsF64) ? 1 : 0;
+    p.group = group;
+    p.rows_per_group = rows_per_group;
+    p.w_group_rows = Cout_pad;
+    p.num_w_groups = num_groups;
+    p.bias_stride = bias_stride;
     return dispatch_gemm(p, block_n, nsplit, stream);
+}
+
+extern "C" int gdrn_conv_fwd(const void* x_hi, const void* x_lo, const void* w_hi, const void* w_lo, void* y_hi,
+                             void* y_lo, float* y_f32, const float* bias, const void* res_hi, const void* res_lo, float* stats,
+                             int N, int H, int W, int Cin, int Cout, int Cout_pad, int KH, int KW, int stride, int pad, int ldc,
+                             int act, int nsplit, void* stream_) {
+    return conv_fwd_impl(x_hi, x_lo, w_hi, w_lo, y_hi, y_lo, y_f32, bias, res_hi, res_lo, stats, N, H, W, Cin, Cout, Cout_pad, KH,
+                         KW, stride, pad, ldc, act, nsplit, nullptr, 0, 1, 0, stream_);
+}
+
+// Class-aware 1x1 output conv: w holds num_groups weight blocks of Cout_pad rows ([num_groups * Cout_pad][K]), bias num_groups
+// blocks of bias_stride floats; output rows [g * rows_per_group, (g + 1) * rows_per_group) use block group[g] (a device array of
+// M / rows_per_group ints, clamped to [0, num_groups)).  No residual and no BatchNorm statistics.
+extern "C" int gdrn_conv_fwd_grouped(const void* x_hi, const void* x_lo, const void* w_hi, const void* w_lo, void* y_hi, void* y_lo,
+                                     float* y_f32, const float* bias, int N, int H, int W, int Cin, int Cout, int Cout_pad, int KH,
+                                     int KW, int stride, int pad, int ldc, int act, int nsplit, const int* group, int rows_per_group,
+                                     int num_groups, int bias_stride, void* stream_) {
+    const int M = N * (H / (stride > 0 ? stride : 1)) * (W / (stride > 0 ? stride : 1));
+    if (int rc = check_groups("conv_fwd_grouped", group, M, rows_per_group, num_groups, bias_stride, bias != nullptr)) return rc;
+    if (act & kActStatsF64) return set_error(GDRN_ERR_ARG, "conv_fwd_grouped: no BatchNorm statistics");
+    return conv_fwd_impl(x_hi, x_lo, w_hi, w_lo, y_hi, y_lo, y_f32, bias, nullptr, nullptr, nullptr, N, H, W, Cin, Cout, Cout_pad, KH,
+                         KW, stride, pad, ldc, act, nsplit, group, rows_per_group, num_groups, bias_stride, stream_);
 }
 
 // Data gradient of a stride-2 convolution (k = 3, pad 1 or k = 1, pad 0), decomposed by OUTPUT PARITY: the pixels
@@ -495,9 +562,9 @@ extern "C" int gdrn_conv_dgrad_s2(const void* du_hi, const void* du_lo, const vo
     return dispatch_gemm(p, block_n, nsplit, stream);
 }
 
-extern "C" int gdrn_gemm_fwd(const void* a_hi, const void* a_lo, const void* w_hi, const void* w_lo, void* y_hi,
-                             void* y_lo, float* y_f32, const float* bias, float* stats, int M, int N, int N_pad, int K,
-                             int ldc, int act, int nsplit, void* stream_) {
+static int gemm_fwd_impl(const void* a_hi, const void* a_lo, const void* w_hi, const void* w_lo, void* y_hi, void* y_lo,
+                         float* y_f32, const float* bias, float* stats, int M, int N, int N_pad, int K, int ldc, int act, int nsplit,
+                         const int* group, int rows_per_group, int num_groups, int bias_stride, void* stream_) {
     cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
     if (nsplit != 1 && nsplit != 3) return set_error(GDRN_ERR_ARG, "gemm_fwd: nsplit must be 1 or 3");
     if (nsplit == 3 && (a_lo == nullptr || w_lo == nullptr)) return set_error(GDRN_ERR_ARG, "gemm_fwd: lo planes missing");
@@ -516,7 +583,7 @@ extern "C" int gdrn_gemm_fwd(const void* a_hi, const void* a_lo, const void* w_h
         uint64_t astr[1] = {(uint64_t)K * 2};
         uint32_t abox[2] = {64, 128};
         if (make_tmap(&p.tmA[pl][0], as[pl], 2, adims, astr, abox)) return GDRN_ERR_CUDA;
-        uint64_t wdims[2] = {(uint64_t)K, (uint64_t)N_pad};
+        uint64_t wdims[2] = {(uint64_t)K, (uint64_t)N_pad * num_groups};
         uint32_t wbox[2] = {64, (uint32_t)block_n};
         if (make_tmap(&p.tmB[pl], ws[pl], 2, wdims, astr, wbox)) return GDRN_ERR_CUDA;
     }
@@ -534,7 +601,30 @@ extern "C" int gdrn_gemm_fwd(const void* a_hi, const void* a_lo, const void* w_h
     p.act = act & ~kActStatsF64;
     p.stats = stats;
     p.stats_f64 = (act & kActStatsF64) ? 1 : 0;
+    p.group = group;
+    p.rows_per_group = rows_per_group;
+    p.w_group_rows = N_pad;
+    p.num_w_groups = num_groups;
+    p.bias_stride = bias_stride;
     return dispatch_gemm(p, block_n, nsplit, stream);
+}
+
+extern "C" int gdrn_gemm_fwd(const void* a_hi, const void* a_lo, const void* w_hi, const void* w_lo, void* y_hi,
+                             void* y_lo, float* y_f32, const float* bias, float* stats, int M, int N, int N_pad, int K,
+                             int ldc, int act, int nsplit, void* stream_) {
+    return gemm_fwd_impl(a_hi, a_lo, w_hi, w_lo, y_hi, y_lo, y_f32, bias, stats, M, N, N_pad, K, ldc, act, nsplit, nullptr, 0, 1, 0,
+                         stream_);
+}
+
+// Grouped plain GEMM (the class-aware output conv's dgrad): w = [num_groups * N_pad][K], rows [g * rows_per_group, ...) of a use
+// weight block group[g] (clamped) and bias + group[g] * bias_stride.  No BatchNorm statistics.
+extern "C" int gdrn_gemm_fwd_grouped(const void* a_hi, const void* a_lo, const void* w_hi, const void* w_lo, void* y_hi, void* y_lo,
+                                     float* y_f32, const float* bias, int M, int N, int N_pad, int K, int ldc, int act, int nsplit,
+                                     const int* group, int rows_per_group, int num_groups, int bias_stride, void* stream_) {
+    if (int rc = check_groups("gemm_fwd_grouped", group, M, rows_per_group, num_groups, bias_stride, bias != nullptr)) return rc;
+    if (act & kActStatsF64) return set_error(GDRN_ERR_ARG, "gemm_fwd_grouped: no BatchNorm statistics");
+    return gemm_fwd_impl(a_hi, a_lo, w_hi, w_lo, y_hi, y_lo, y_f32, bias, nullptr, M, N, N_pad, K, ldc, act, nsplit, group,
+                         rows_per_group, num_groups, bias_stride, stream_);
 }
 
 // BLOCK_N * 10 + NSPLIT of the most recent gdrn_conv_fwd / gdrn_gemm_fwd call on this thread

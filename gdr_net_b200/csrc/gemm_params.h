@@ -34,6 +34,10 @@ struct GemmParams {
     int ph_a[4], ph_b[4];
     signed char tap_dh[12], tap_dw[12], tap_w[12];
     int pw_log2, ph_log2;  // log2 of the dY width / height
+    // Grouped variant (gemm_fwd_grouped_kernel only): output rows [g * rows_per_group, (g + 1) * rows_per_group) use weight rows
+    // [group[g] * w_group_rows, ...) and bias + group[g] * bias_stride; group[g] is clamped to [0, num_w_groups).
+    const int* group;
+    int rows_per_group, w_group_rows, num_w_groups, bias_stride;
 };
 
 }  // namespace gdrn

@@ -93,6 +93,39 @@ def pose_loss_switches(pnp_cfg) -> tuple:
     return sw, names
 
 
+def check_roi_classes(roi_classes, B: int, num_classes: int):
+    """ValueError unless roi_classes holds B integer class indices in [0, num_classes) (reference GDRN.py:134-151 asserts that
+    they are given and indexes with them).  Costs one small device-to-host copy when they live on the device."""
+    if roi_classes is None:
+        raise ValueError("roi_classes is required: the geometry head is class-aware (ROT_HEAD.*_CLASS_AWARE)")
+    c = torch.as_tensor(roi_classes)
+    if c.dtype.is_floating_point or c.dtype.is_complex or c.dtype == torch.bool:
+        raise ValueError(f"roi_classes: expected integer class indices, got {c.dtype}")
+    if c.numel() != B:
+        raise ValueError(f"roi_classes: expected {B} class indices, got shape {tuple(c.shape)}")
+    lo, hi = torch.stack([c.min(), c.max()]).tolist()
+    if lo < 0 or hi >= num_classes:
+        raise ValueError(f"roi_classes: class indices must lie in [0, NUM_CLASSES = {num_classes}), got [{lo}, {hi}]")
+    return c
+
+
+def class_rows(num_classes: int, mo: int, num_regions: int, rot_aware: bool, mask_aware: bool, region_aware: bool):
+    """(rows, n_rows): rows[c] lists the output-conv rows of class c in the engine's logit order (mask | x y z | bg | R regions),
+    n_rows the output conv's row count.  The reference's layout (cdpn_rot_head_region.py:114-135, 186-193; GDRN.py:134-151):
+    [mask, MO per class if MASK_CLASS_AWARE] [x_0..x_{C-1} | y_0.. | z_0.. if ROT_CLASS_AWARE, else x y z] [bg + R regions, per
+    class if REGION_CLASS_AWARE]; a block that is not class-aware is shared by every class."""
+    cm, cr, cg = (num_classes if mask_aware else 1), (num_classes if rot_aware else 1), (num_classes if region_aware else 1)
+    xyz0 = mo * cm
+    reg0 = xyz0 + 3 * cr
+    rows = []
+    for c in range(num_classes):
+        r = [(c if mask_aware else 0) * mo + j for j in range(mo)]
+        r += [xyz0 + a * cr + (c if rot_aware else 0) for a in range(3)]
+        r += [reg0 + (c if region_aware else 0) * (num_regions + 1) + j for j in range(num_regions + 1)]
+        rows.append(r)
+    return rows, reg0 + (num_regions + 1) * cg
+
+
 class _BN:
     """Per-BatchNorm scratch: scale/shift (forward), mean/invstd (backward), statistic slices."""
 
@@ -193,9 +226,17 @@ class Engine:
         # mask head (GDRN.py:339-400): MASK_LOSS_TYPE, the mask logits per pixel (1, or 2 for CE) and the GT mask of the xyz, mask
         # and region losses (XYZ_LOSS_MASK_GT, MASK_LOSS_GT, REGION_LOSS_MASK_GT)
         self.mask_loss = MASK_LOSSES[rh.MASK_LOSS_TYPE]
-        self.n_logits = model.rot_head_net.features[23].out_channels  # mask | xyz | bg | R regions
-        self.mask_out = self.n_logits - 4 - self.num_regions
-        assert self.mask_out == (2 if self.mask_loss == MASK_LOSSES["CE"] else 1), (self.mask_loss, self.mask_out)
+        self.mask_out = 2 if self.mask_loss == MASK_LOSSES["CE"] else 1
+        self.n_logits = self.mask_out + 4 + self.num_regions  # per crop: mask | xyz | bg | R regions
+        # class-aware head (ROT_HEAD.*_CLASS_AWARE): the output conv holds per-class rows (class_rows) and every crop's logits come
+        # from its class's rows, selected per 128-row tile by the grouped GEMMs -- the logit row layout stays the one above
+        aware = (bool(rh.ROT_CLASS_AWARE), bool(rh.MASK_CLASS_AWARE), bool(rh.REGION_CLASS_AWARE))
+        self.class_aware = any(aware)
+        self.num_classes = int(rh.NUM_CLASSES) if self.class_aware else 1
+        rows, n_rows = class_rows(self.num_classes, self.mask_out, self.num_regions, *aware)
+        assert model.rot_head_net.features[23].out_channels == n_rows, (model.rot_head_net.features[23].out_channels, n_rows)
+        if self.class_aware:
+            self._init_class_tables(rows, n_rows)
         self.mask_gt = (rh.XYZ_LOSS_MASK_GT, rh.MASK_LOSS_GT, rh.REGION_LOSS_MASK_GT)
         # pose losses (PNP_NET switches): the shipped set runs gdrn_pose_loss (8 losses, LOSS_NAMES), any other gdrn_pose_loss_ex
         sw, pose_names = pose_loss_switches(model.cfg.MODEL.CDPN.PNP_NET)
@@ -250,6 +291,34 @@ class Engine:
 
         self._seg = segment_bounds(self.named_params, SEGMENTS)
 
+    def _init_class_tables(self, rows, n_rows):
+        """Device tables of the class-aware head: cls_idx [C * cls_npad] = the output-conv row behind each slot of the class-major
+        weight table (-1: zero padding), cls_slot [C][n_rows] = the logit slot of each row for each class (-1: not used by it),
+        and the persistent class-major fp32 tables w_cls [C * cls_npad][256] / b_cls that every step gathers and packs."""
+        import numpy as np
+
+        C_, npad = self.num_classes, -(-self.n_logits // 64) * 64
+        idx = np.full(C_ * npad, -1, dtype=np.int32)
+        slot = np.full((C_, n_rows), -1, dtype=np.int32)
+        for c, r in enumerate(rows):
+            idx[c * npad:c * npad + len(r)] = r
+            slot[c, r] = np.arange(len(r))
+        self.cls_npad, self.cls_rows = npad, n_rows
+        self.cls_idx = torch.from_numpy(idx).to(self.dev)
+        self.cls_slot = torch.from_numpy(slot).to(self.dev)
+        self.w_cls = torch.zeros(C_ * npad, 256, device=self.dev)
+        self.b_cls = torch.zeros(C_ * npad, device=self.dev)
+
+    def _classes(self, roi_classes, B: int) -> torch.Tensor:
+        """roi_classes [B] (any integer dtype, host or device; GDRN.forward checked the range) -> int32 [B] on the device.  The
+        kernels clamp a class outside [0, NUM_CLASSES) to the nearest table entry instead of reading outside the tables."""
+        if roi_classes is None:
+            raise ValueError("roi_classes is required: the geometry head is class-aware (ROT_HEAD.*_CLASS_AWARE)")
+        c = torch.as_tensor(roi_classes)
+        if c.numel() != B:
+            raise ValueError(f"roi_classes: expected {B} class indices, got shape {tuple(c.shape)}")
+        return c.reshape(B).to(self.dev, torch.int32).contiguous()
+
     # ------------------------------------------------------------------------------------------ weights
     def _conv_modules(self):
         """(key, module) of every conv packed by pack_conv_fwd; the 7x7 stem is a GEMM over its im2col matrix (pack_stem)."""
@@ -283,6 +352,11 @@ class Engine:
         with torch.no_grad():
             torch.cat([self.model.pnp_net.fc_r.weight, self.model.pnp_net.fc_t.weight], 0, out=self.w_rt)
             torch.cat([self.model.pnp_net.fc_r.bias, self.model.pnp_net.fc_t.bias], 0, out=self.b_rt)
+        if self.class_aware:  # the class-major tables the pack jobs of the output conv read
+            w23 = self.model.rot_head_net.features[23]
+            n = self.num_classes * self.cls_npad
+            C.gdrn_class_gather(w23.weight.data_ptr(), self.cls_idx.data_ptr(), self.w_cls.data_ptr(), n, 256, self.cls_rows, _stream())
+            C.gdrn_class_gather(w23.bias.data_ptr(), self.cls_idx.data_ptr(), self.b_cls.data_ptr(), n, 1, self.cls_rows, _stream())
         C.gdrn_pack_weight_batched(tab["jobs"].data_ptr(), tab["njobs"], tab["blocks"], _stream())
 
     def _pack_table(self, pack, row_scales=None) -> dict:
@@ -432,8 +506,12 @@ class Engine:
         of the three FC layers; pnp_saved receives the Patch-PnP conv activations (pnp_net_forward)."""
         m, B, dev = self.model, head_in.shape[0], self.dev
         logits = torch.empty(B * 4096, 72, device=dev)
-        ops.conv_fwd(head_in, self.wf["rot_head_net.features.23"], self.n_logits, 1, 1, 1, 0, out_f32=logits,
-                     bias=m.rot_head_net.features[23].bias, ldc=72, want_planes=False)
+        if self.class_aware:  # crop b (4096 rows) reads the weight / bias block of class roi_classes[b]
+            ops.conv_fwd_grouped(head_in, self.wf["rot_head_net.features.23"], self.n_logits, self.cls_npad, aux["roi_classes"], 4096,
+                                 out_f32=logits, bias=self.b_cls, bias_stride=self.cls_npad, ldc=72)
+        else:
+            ops.conv_fwd(head_in, self.wf["rot_head_net.features.23"], self.n_logits, 1, 1, 1, 0, out_f32=logits,
+                         bias=m.rot_head_net.features[23].bias, ldc=72, want_planes=False)
         pnp_in = PT((B, 64, 64, self.pnp_ld), self.planes, device=dev)
         glue = (logits.data_ptr(), ops.ptr(aux.get("roi_coord_2d")), aux["roi_extents"].data_ptr(), pnp_in.hi_ptr, pnp_in.lo_ptr, B, 4096,
                 self.with_2d, self.mask_out)
@@ -467,6 +545,9 @@ class Engine:
         m, pl, bpl = self.model, self.planes, self.bplanes
         wf, wd = self.wf, self.wd
         for key, conv in self._conv_modules():
+            if key == "rot_head_net.features.23" and self.class_aware:
+                self._class_head_pack_calls(need_dgrad)
+                continue
             wf[key] = ops.pack_conv_fwd(conv.weight, pl, out=wf.get(key))
             if need_dgrad:
                 # the logit gradient of head_bwd is 128 columns wide whatever the output conv's row count (MO + 4 + R)
@@ -490,6 +571,17 @@ class Engine:
             wd["fc2"] = ops.pack_linear(pn.fc2.weight, bpl, out=wd.get("fc2"), transpose=True)
             wd["fc_rt"] = ops.pack_linear(self.w_rt, bpl, out=wd.get("fc_rt"), transpose=True)
         wf["stem"] = ops.pack_stem(m.backbone.conv1.weight, pl, out=wf.get("stem"))
+
+    def _class_head_pack_calls(self, need_dgrad: bool):
+        """Class-aware output conv: forward operand [C * cls_npad][256] and dgrad operand [C][256][128] from the class-major table."""
+        key, C_, npad = "rot_head_net.features.23", self.num_classes, self.cls_npad
+        src = self.w_cls.view(C_ * npad, 256, 1, 1)
+        self.wf[key] = ops.pack_conv_fwd(src, self.planes, out=self.wf.get(key))
+        if need_dgrad:
+            wd = self.wd.get(key) or PT((C_ * 256, 128), self.bplanes, device=self.dev)
+            self.wd[key] = wd
+            for c in range(C_):
+                ops.pack_conv_dgrad(src[c * npad:(c + 1) * npad], self.bplanes, out=_PlaneRows(wd, c * 256), ipad=128)
 
     # ------------------------------------------------------------------------------------------ building blocks
     def _bn_fwd(self, key: str, u: PT, relu: bool, train_bn: bool, res: Optional[PT] = None) -> PT:
@@ -531,7 +623,7 @@ class Engine:
         return u, self._bn_fwd(bkey, u, relu, train_bn, res)
 
     # ------------------------------------------------------------------------------------------ forward
-    def run(self, x, *, roi_coord_2d, roi_cams, roi_centers, roi_whs, roi_extents, resize_ratios, gt_xyz=None,
+    def run(self, x, *, roi_coord_2d, roi_cams, roi_centers, roi_whs, roi_extents, resize_ratios, roi_classes=None, gt_xyz=None,
             gt_mask_trunc=None, gt_mask_visib=None, gt_mask_obj=None, gt_region=None, gt_ego_rot=None, gt_points=None,
             sym_infos=None, gt_trans=None, gt_trans_ratio=None, do_loss=False, train_bn=False, want_maps=False):
         aux = dict(roi_coord_2d=roi_coord_2d, roi_cams=roi_cams, roi_centers=roi_centers, roi_whs=roi_whs,
@@ -564,6 +656,8 @@ class Engine:
                 raise ValueError(f"sym_infos: expected a list of {B} entries, got {len(aux['sym_infos'])}")
             aux["sym_idx"] = self.sym_table.indices(aux["sym_infos"])  # the matrices themselves are already on the device
         aux.pop("sym_infos", None)
+        if self.class_aware:  # device data: a captured graph reads the classes of each replay from its static copy
+            aux["roi_classes"] = self._classes(roi_classes, B)
         x = x.to(self.dev).float().contiguous()
         if not do_loss:
             with torch.no_grad():
@@ -823,15 +917,18 @@ class Engine:
         hf = m.rot_head_net.features
         head_in = h(S["head_in"])
         n_out = self.n_logits  # rows of the 1x1 output conv
-        def head_out_wgrad():
-            buf, ks, kss = ops.gemm_wgrad(dlog, head_in.view(B * 4096, 256), self.ws)
-            ops.unpack_wgrad(buf, self.grads["rot_head_net.features.23.weight"], n_out, 256, 1, 1, 256, ks, kss, 256, 1, 0, 0)
+        if self.class_aware:
+            g = self._class_head_bwd(dlog, head_in, aux["roi_classes"], B)
+        else:
+            def head_out_wgrad():
+                buf, ks, kss = ops.gemm_wgrad(dlog, head_in.view(B * 4096, 256), self.ws)
+                ops.unpack_wgrad(buf, self.grads["rot_head_net.features.23.weight"], n_out, 256, 1, 1, 256, ks, kss, 256, 1, 0, 0)
 
-        self._on_side(head_out_wgrad, keep=(dlog,))
-        tmp128 = torch.empty(128, device=dev)
-        C.gdrn_colsum(dlog.hi_ptr, dlog.lo_ptr, tmp128.data_ptr(), B * 4096, 128, _stream())
-        self.grads["rot_head_net.features.23.bias"].copy_(tmp128[:n_out])
-        g = ops.gemm_fwd(dlog, self.wd["rot_head_net.features.23"], 256).view(B, 64, 64, 256)
+            self._on_side(head_out_wgrad, keep=(dlog,))
+            tmp128 = torch.empty(128, device=dev)
+            C.gdrn_colsum(dlog.hi_ptr, dlog.lo_ptr, tmp128.data_ptr(), B * 4096, 128, _stream())
+            self.grads["rot_head_net.features.23.bias"].copy_(tmp128[:n_out])
+            g = ops.gemm_fwd(dlog, self.wd["rot_head_net.features.23"], 256).view(B, 64, 64, 256)
 
         # ---- head convs (cdpn_rot_head_region.py:95-125)
         for L in reversed(S["head"]):
@@ -886,6 +983,23 @@ class Engine:
         self.saved = None
         return self.grads
 
+    def _class_head_bwd(self, dlog: PT, head_in: PT, classes: torch.Tensor, B: int) -> PT:
+        """Backward of the class-aware output conv: the grouped dgrad on the main stream; on the side stream the per-crop weight
+        partials (the wgrad GEMM split at crop boundaries, ksplit = B) and per-crop bias partials, reduced in crop order into the
+        reference layout (rows of classes absent from the batch get exactly 0)."""
+        def work():
+            buf, ks, kss = ops.gemm_wgrad(dlog, head_in.view(B * 4096, 256), self.ws, ksplit=B)
+            assert ks == B, (ks, B)  # 4096 rows = 64 k-blocks per split: split b is crop b
+            bias_part = torch.empty(B, 128, device=self.dev)
+            C.gdrn_crop_colsum(dlog.hi_ptr, dlog.lo_ptr, bias_part.data_ptr(), B, 4096, 128, _stream())
+            C.gdrn_class_wgrad_reduce(buf.data_ptr(), kss, 256, bias_part.data_ptr(), 128, classes.data_ptr(), B,
+                                      self.cls_slot.data_ptr(), self.num_classes, self.cls_rows, self.n_logits, 256,
+                                      self.grads["rot_head_net.features.23.weight"].data_ptr(),
+                                      self.grads["rot_head_net.features.23.bias"].data_ptr(), _stream())
+
+        self._on_side(work, keep=(dlog, classes))
+        return ops.gemm_fwd_grouped(dlog, self.wd["rot_head_net.features.23"], 256, classes, 4096).view(B, 64, 64, 256)
+
     def materialize_aliased_grads(self):
         """A p.grad that still aliases flat_grad (adopted by autograd in an earlier step and not reset by zero_grad) would be
         overwritten by the next backward: give such gradients their own storage first (gradient accumulation stays exact)."""
@@ -915,6 +1029,15 @@ class Engine:
         out = ops.like(g)
         C.gdrn_leaky_bwd(g.hi_ptr, g.lo_ptr, y.hi_ptr, out.hi_ptr, out.lo_ptr, g.numel(), _stream())
         return out
+
+
+class _PlaneRows:
+    """Rows [r0, ...) of a PT as a pack destination (the per-class blocks of the class-aware dgrad operand)."""
+
+    def __init__(self, pt: PT, r0: int):
+        self.pt = pt
+        self.hi_ptr = pt.buf[0, r0].data_ptr()
+        self.lo_ptr = pt.buf[1, r0].data_ptr() if pt.planes == 2 else None
 
 
 def _capture_mode():

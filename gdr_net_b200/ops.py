@@ -256,6 +256,27 @@ def gemm_fwd(a: PT, wp: PT, N: int, *, out: PT | None = None, out_f32: torch.Ten
     return out
 
 
+def conv_fwd_grouped(x: PT, wp: PT, Cout: int, Cout_pad: int, group: torch.Tensor, rows_per_group: int, *, out_f32: torch.Tensor,
+                     bias=None, bias_stride: int = 0, ldc: int | None = None):
+    """1x1 / k x k stride-1 conv whose output rows [g * rows_per_group, ...) use weight block group[g] of wp ([G * Cout_pad][K]) and
+    bias[group[g] * bias_stride:]; group: int32 device tensor.  fp32 output only (the class-aware output conv's logits)."""
+    N, H, W, Cin = x.shape
+    G = wp.shape[0] // Cout_pad
+    C.gdrn_conv_fwd_grouped(x.hi_ptr, x.lo_ptr, wp.hi_ptr, wp.lo_ptr, None, None, out_f32.data_ptr(), ptr(bias), N, H, W, Cin, Cout,
+                            Cout_pad, 1, 1, 1, 0, ldc or _round_up(Cout, 64), 0, x.nsplit, group.data_ptr(), rows_per_group, G,
+                            bias_stride, _stream())
+
+
+def gemm_fwd_grouped(a: PT, wp: PT, N: int, group: torch.Tensor, rows_per_group: int) -> PT:
+    """y = a w_g^T with w_g = block group[row // rows_per_group] of wp ([G * N][K], N % 64 == 0): the class-aware dgrad."""
+    M, K = a.shape
+    G = wp.shape[0] // N
+    out = PT((M, N), a.planes, device=a.buf.device)
+    C.gdrn_gemm_fwd_grouped(a.hi_ptr, a.lo_ptr, wp.hi_ptr, wp.lo_ptr, out.hi_ptr, out.lo_ptr, None, None, M, N, N, K, N, 0, a.nsplit,
+                            group.data_ptr(), rows_per_group, G, 0, _stream())
+    return out
+
+
 class Workspace:
     """Grow-only fp32 scratch for split-K weight-gradient partials."""
 

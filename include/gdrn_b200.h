@@ -65,6 +65,30 @@ int gdrn_gemm_fwd(const void* a_hi, const void* a_lo, const void* w_hi, const vo
                   float* y_f32, const float* bias, float* stats, int M, int N, int N_pad, int K, int ldc, int act,
                   int nsplit, void* stream);
 
+/* ---- class-aware output conv (ROT_HEAD.*_CLASS_AWARE; GDRN.py:134-151, cdpn_rot_head_region.py:114-135): grouped GEMMs.
+ * w holds num_groups blocks of Cout_pad (N_pad) rows, [num_groups * Cout_pad][K]; bias num_groups blocks of bias_stride floats.
+ * Output rows [g * rows_per_group, (g + 1) * rows_per_group) use block group[g] (device int array of M / rows_per_group entries,
+ * clamped to [0, num_groups)); rows_per_group % 128 == 0, so no 128-row tile straddles two groups.  No residual, no statistics. */
+int gdrn_conv_fwd_grouped(const void* x_hi, const void* x_lo, const void* w_hi, const void* w_lo, void* y_hi, void* y_lo,
+                          float* y_f32, const float* bias, int N, int H, int W, int Cin, int Cout, int Cout_pad, int KH, int KW,
+                          int stride, int pad, int ldc, int act, int nsplit, const int* group, int rows_per_group, int num_groups,
+                          int bias_stride, void* stream);
+int gdrn_gemm_fwd_grouped(const void* a_hi, const void* a_lo, const void* w_hi, const void* w_lo, void* y_hi, void* y_lo,
+                          float* y_f32, const float* bias, int M, int N, int N_pad, int K, int ldc, int act, int nsplit,
+                          const int* group, int rows_per_group, int num_groups, int bias_stride, void* stream);
+/* dst[i][k] = src[idx[i]][k], 0 where idx[i] is outside [0, n_src): the per-step class-major weight / bias tables */
+int gdrn_class_gather(const float* src, const int* idx, float* dst, int n_dst, int K, int n_src, void* stream);
+/* out[b][c] = sum of rows [b * rows_per_crop, (b + 1) * rows_per_crop) of column c of a [B * rows_per_crop][ld] planar tensor,
+ * in a fixed order (the per-crop bias partials of the class-aware output conv) */
+int gdrn_crop_colsum(const void* x_hi, const void* x_lo, float* out, int B, int rows_per_crop, int ld, void* stream);
+/* Weight and bias gradients of the class-aware output conv from per-crop partials: ws [B] blocks of ws_crop_stride floats holding
+ * [n_slots][ws_ld] (gdrn_gemm_wgrad with ksplit = B), bias_part [B][bias_ld] (gdrn_crop_colsum).  For every reference row r < n_rows
+ * grad_w[r][k] = sum over b in crop order of ws[b][slot_of[c_b][r]][k] (grad_b likewise), where c_b = classes[b] clamped to
+ * [0, num_classes) and slot_of [num_classes][n_rows] is the logit slot of row r for class c or -1: rows no crop uses get 0. */
+int gdrn_class_wgrad_reduce(const float* ws, long ws_crop_stride, int ws_ld, const float* bias_part, int bias_ld,
+                            const int* classes, int B, const int* slot_of, int num_classes, int n_rows, int n_slots, int K,
+                            float* grad_w, float* grad_b, void* stream);
+
 /* ---- weight gradients (autograd wgrad of the layers above).  Split-K partials are written to the fp32
  * workspace ws [ksplit][ceil(Cout/128)*128][KH*KW*Cin]; reduce with gdrn_unpack_wgrad.
  * ws == NULL: size query only (*ws_need_out floats, *ksplit_out). ksplit <= 0: automatic. */
