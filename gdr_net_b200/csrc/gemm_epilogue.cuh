@@ -18,9 +18,20 @@ namespace gdrn {
 // rebuilt from the kernel parameters for every chunk: unsigned arithmetic keeps the compiler from hoisting them into 64-bit
 // per-row pointers, which would not fit next to the accumulators of a 128-wide 3-pass tile.
 // GROUPED: the bias of this tile starts at p.bias + bias_off (the tile's weight group, gemm_fwd_grouped_kernel).
-template <int BLOCK_N, bool GROUPED = false>
+// STAGED: the 16-bit planes are not stored here but written to this warpgroup's staging area `stg` in shared memory (plane p at
+//          stg + p * (J1 - J0) * 1024: one 128-byte-swizzled [64 rows][64 columns] box per 64 columns, 8 KB apart), from where
+//          the kernel stores them with TMA.  fp32 outputs are always stored here.
+// J0, J1 : the column groups (8 columns each) of this call; a 128-wide 3-pass tile is staged in two 64-column halves.
+// Staging slot of (column group j, row half h) of this thread's first plane: row r of a box keeps its 16-byte column chunk c at
+// chunk c ^ (r % 8) (SWIZZLE_128B); the 8 rows of a warp's store have distinct r % 8, so the 32 lanes hit 32 distinct banks.
+__device__ __forceinline__ uint32_t* stage_slot(uint8_t* stg, int row0, int lane, int j, int h) {
+    return reinterpret_cast<uint32_t*>(stg + (row0 & 63) * 128 + 4 * (lane & 3) + (j >> 3) * 8192 + (((j & 7) ^ (row0 & 7)) << 4) +
+                                       h * 1024);
+}
+
+template <int BLOCK_N, bool GROUPED = false, bool STAGED = false, int J0 = 0, int J1 = BLOCK_N / 8>
 __device__ __forceinline__ void gemm_epilogue_tile(const GemmParams& p, const float* acc, int lane, int row0, int m_tile, int n_tile,
-                                                   int ph, float* s_stats, int bias_off = 0) {
+                                                   int ph, float* s_stats, int bias_off = 0, uint8_t* stg = nullptr) {
     __nv_bfloat16* out_hi = reinterpret_cast<__nv_bfloat16*>(p.out_hi);
     __nv_bfloat16* out_lo = reinterpret_cast<__nv_bfloat16*>(p.out_lo);
     const __nv_bfloat16* res_hi = reinterpret_cast<const __nv_bfloat16*>(p.res_hi);
@@ -43,7 +54,7 @@ __device__ __forceinline__ void gemm_epilogue_tile(const GemmParams& p, const fl
         off[h] = grow * (uint32_t)p.ldc + (uint32_t)(n_tile * BLOCK_N + 2 * q);
     }
 #pragma unroll
-    for (int j = 0; j < BLOCK_N / 8; ++j) {
+    for (int j = J0; j < J1; ++j) {
         const int cl = 8 * j + 2 * q;  // column inside the tile
         const int col = n_tile * BLOCK_N + cl;
         if (n_tile * BLOCK_N + 32 * (j / 4) >= p.N) continue;  // warp-uniform: chunk beyond N
@@ -86,6 +97,22 @@ __device__ __forceinline__ void gemm_epilogue_tile(const GemmParams& p, const fl
                 if (p.act == 1) f[h][e] = f[h][e] > 0.f ? f[h][e] : 0.1f * f[h][e];
                 else if (p.act == 2) f[h][e] = fmaxf(f[h][e], 0.f);
             }
+        if constexpr (STAGED) {
+            // rows beyond M and columns beyond the output map's width are clipped by the TMA store
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                const float a = ok0 ? f[h][0] : 0.f, b = ok1 ? f[h][1] : 0.f;
+                uint32_t* const d = stage_slot(stg, row0, lane, j - J0, h);
+                uint32_t hi, lo;
+                if (out_lo != nullptr) {
+                    split2(a, b, hi, lo);
+                    d[(J1 - J0) * 256] = lo;  // the lo plane, (J1 - J0) * 1024 bytes on
+                } else {
+                    hi = pack_hi2(a, b);
+                }
+                *d = hi;
+            }
+        }
         if (col < p.ldc) {  // ldc % 8 == 0: the pair (col, col + 1) is inside or outside together
 #pragma unroll
             for (int h = 0; h < 2; ++h) {
@@ -93,7 +120,7 @@ __device__ __forceinline__ void gemm_epilogue_tile(const GemmParams& p, const fl
                 const float a = ok0 ? f[h][0] : 0.f, b = ok1 ? f[h][1] : 0.f;
                 const uint32_t o = off[h] + 8 * j;
                 if (p.out_f32 != nullptr) *reinterpret_cast<float2*>(p.out_f32 + o) = make_float2(a, b);
-                if (out_hi != nullptr) {
+                if (!STAGED && out_hi != nullptr) {
                     uint32_t hi, lo;
                     if (out_lo != nullptr) {
                         split2(a, b, hi, lo);

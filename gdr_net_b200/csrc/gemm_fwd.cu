@@ -16,7 +16,9 @@
 //   * warpgroups 0 and 1 = MMA + epilogue, each owning 64 of the 128 rows of a tile (wgmma m64nNk16,
 //     accumulators in registers; the epilogue in gemm_epilogue.cuh applies bias / residual / activation,
 //     stores 16-bit hi[/lo] or fp32 and accumulates the per-channel BatchNorm statistics).  While the MMA
-//     warpgroups run a tile's epilogue the producer already fills the stages of the next tile.
+//     warpgroups run a tile's epilogue the producer already fills the stages of the next tile.  gemm_fwd_tma_kernel (every
+//     launch with a 16-bit output but the phase dgrads, make_out_maps) instead stages the 16-bit planes in a shared-memory buffer
+//     behind the ring and writes them with TMA stores, so the MMAs of the next tile start while the tile drains.
 //     Warp 8 = TMA producer.  With nine warps ptxas allots at most 168 registers per thread (three warps share one SM
 //     sub-partition's register file).  A 128-wide 3-pass tile holds 128 accumulator registers (main + cross) in its main
 //     loop; it fits (ptxas -v: 162 registers, no spills) because the cross accumulator is folded into the main one before
@@ -50,6 +52,13 @@ struct GemmCfg {
     static constexpr int STAGES_RAW = (kSmemBudget - kAuxBytes - 1024) / STAGE_BYTES;
     static constexpr int STAGES = STAGES_RAW > 8 ? 8 : STAGES_RAW;
     static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + kAuxBytes + 1024;
+    // gemm_fwd_tma_kernel: a 32 KB output staging buffer behind the ring (16 KB per MMA warpgroup: its 64 rows of one 128-wide or
+    // two 64-wide 16-bit planes), paid for by a smaller aux area (barriers at +0, the [2][BLOCK_N] partial sums at +512); the ring
+    // keeps its stages.
+    static constexpr int OUT_STAGE_BYTES = 32768;
+    static constexpr int SMEM_BYTES_TMA = STAGES * STAGE_BYTES + OUT_STAGE_BYTES + 2048 + 1024;
+    static_assert(SMEM_BYTES_TMA <= kSmemBudget, "no room for the output staging buffer");
+    static_assert(512 + 2 * BLOCK_N * 4 <= 2048 && 2 * STAGES * 8 <= 512, "aux area of gemm_fwd_tma_kernel");
     // 3-pass mode: the small cross terms (hi*lo + lo*hi) are kept in their own accumulator and added to the main one with a
     // round-to-nearest fp32 fma before the epilogue.  Each k-step issues three MMAs of width BLOCK_N, each writing one WHOLE
     // accumulator: a_hi x [w_hi; w_lo] as one 2 * BLOCK_N-wide MMA followed by a_lo x w_hi into its upper half would read
@@ -67,7 +76,7 @@ __device__ __forceinline__ int tile_group(const GemmParams& p, int m_tile) {
     return min(max(g, 0), p.num_w_groups - 1);
 }
 
-template <int BLOCK_N, int NSPLIT, bool GROUPED>
+template <int BLOCK_N, int NSPLIT, bool GROUPED, bool OUT_TMA>
 __device__ __forceinline__ void gemm_fwd_body(const GemmParams& p) {
     using Cfg = GemmCfg<BLOCK_N, NSPLIT>;
     constexpr int NPL = Cfg::NPL;
@@ -77,7 +86,7 @@ __device__ __forceinline__ void gemm_fwd_body(const GemmParams& p) {
     // shared address space, so the epilogue's statistics compile to shared-memory atomics instead of generic ones
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-    uint8_t* aux = smem + STAGES * Cfg::STAGE_BYTES;
+    uint8_t* aux = smem + STAGES * Cfg::STAGE_BYTES + (OUT_TMA ? Cfg::OUT_STAGE_BYTES : 0);
     uint64_t* full_bar = reinterpret_cast<uint64_t*>(aux);
     uint64_t* empty_bar = full_bar + STAGES;
     float* s_stats = reinterpret_cast<float*>(aux + 512);  // [2][BLOCK_N]
@@ -91,6 +100,7 @@ __device__ __forceinline__ void gemm_fwd_body(const GemmParams& p) {
         for (int pl = 0; pl < NPL; ++pl) {
             tma_prefetch_desc(&p.tmB[pl]);
             tma_prefetch_desc(&p.tmA[pl][0]);
+            if constexpr (OUT_TMA) tma_prefetch_desc(&p.tmC[pl]);
         }
         for (int s = 0; s < STAGES; ++s) {
             mbar_init(&full_bar[s], 1);
@@ -209,6 +219,18 @@ __device__ __forceinline__ void gemm_fwd_body(const GemmParams& p) {
     const int cch = p.cchunks, nph = p.nphase, nkb_all = p.num_kb;
     int stage = 0;
     uint32_t phase = 0;
+    // TMA-stored output: each warpgroup stages its 64 rows of the 16-bit planes in its own 16 KB half of the staging buffer
+    // ([plane][64-column box][64 rows][128 B]) and one thread stores them with TMA while the warpgroup goes on to the next tile's
+    // MMAs; the buffer is rewritten only after those stores have read it, normally a whole tile later.  The two planes of a
+    // 128-wide 3-pass tile (32 KB) are staged in two 64-column halves, the second once the first half's stores have read the buffer.
+    constexpr int PASSES = (BLOCK_N == 128 && NSPLIT == 3) ? 2 : 1;
+    constexpr int JP = BLOCK_N / 8 / PASSES;  // column groups per pass
+    static_assert(JP * 1024 * NPL <= Cfg::OUT_STAGE_BYTES / 2, "staging buffer too small");
+    uint8_t* const stg = smem + STAGES * Cfg::STAGE_BYTES + cw * (Cfg::OUT_STAGE_BYTES / 2);
+    auto wg_sync = [&]() {
+        if (cw == 0) named_bar_sync<3, 128>();
+        else named_bar_sync<4, 128>();
+    };
     for (int grp = my_cta; grp < num_groups; grp += num_ctas) {
         int rem = grp, ph = 0, nkb = nkb_all;
         if (nph) {
@@ -260,13 +282,40 @@ __device__ __forceinline__ void gemm_fwd_body(const GemmParams& p) {
                 asm volatile("" : "+f"(acc[i]));
             }
         }
+        const int row0 = cw * 64 + (warp & 3) * 16 + (lane >> 2);
         if constexpr (GROUPED) {
-            gemm_epilogue_tile<BLOCK_N, true>(p, acc, lane, cw * 64 + (warp & 3) * 16 + (lane >> 2), m_tile, n_tile, ph, s_stats,
-                                              tile_group(p, m_tile) * p.bias_stride);
+            gemm_epilogue_tile<BLOCK_N, true>(p, acc, lane, row0, m_tile, n_tile, ph, s_stats, tile_group(p, m_tile) * p.bias_stride);
+        } else if constexpr (OUT_TMA) {
+            const int grow0 = m_tile * kBlockM + cw * 64;  // first output row of this warpgroup
+            auto store = [&](int box0) {                   // one thread: the staged boxes of both planes
+                if (grow0 < p.M) {
+                    for (int pl = 0; pl < (p.out_lo != nullptr ? 2 : 1); ++pl)
+                        for (int b = 0; b < JP / 8; ++b)
+                            if (n_tile * BLOCK_N + 64 * (box0 + b) < p.N)
+                                tma_store_2d_u32(reinterpret_cast<uint64_t>(&p.tmC[pl]), smem_u32(stg) + (pl * (JP / 8) + b) * 8192,
+                                                 n_tile * BLOCK_N + 64 * (box0 + b), grow0);
+                }
+                bulk_commit_group();
+            };
+            if (signaller) bulk_wait_group_read<0>();  // the previous stores have read the buffer
+            wg_sync();
+            gemm_epilogue_tile<BLOCK_N, false, true, 0, JP>(p, acc, lane, row0, m_tile, n_tile, ph, s_stats, 0, stg);
+            fence_proxy_async();  // this thread's st.shared -> visible to the TMA store (async proxy)
+            wg_sync();
+            if (signaller) store(0);
+            if constexpr (PASSES == 2) {
+                if (signaller) bulk_wait_group_read<0>();
+                wg_sync();
+                gemm_epilogue_tile<BLOCK_N, false, true, JP, 2 * JP>(p, acc, lane, row0, m_tile, n_tile, ph, s_stats, 0, stg);
+                fence_proxy_async();
+                wg_sync();
+                if (signaller) store(JP / 8);
+            }
         } else {
-            gemm_epilogue_tile<BLOCK_N>(p, acc, lane, cw * 64 + (warp & 3) * 16 + (lane >> 2), m_tile, n_tile, ph, s_stats);
+            gemm_epilogue_tile<BLOCK_N>(p, acc, lane, row0, m_tile, n_tile, ph, s_stats);
         }
     }
+    if (OUT_TMA && signaller) bulk_wait_group<0>();  // the output is written before the CTA exits
     if (p.stats != nullptr) {
         asm volatile("bar.sync 1, 256;" ::: "memory");  // the two MMA warpgroups only
         const int n_tile = my_cta % p.num_n_tiles;      // fixed per CTA (num_ctas % num_n_tiles == 0)
@@ -287,13 +336,19 @@ __device__ __forceinline__ void gemm_fwd_body(const GemmParams& p) {
 
 template <int BLOCK_N, int NSPLIT>
 __global__ void __launch_bounds__(kThreads, 1) gemm_fwd_kernel(const __grid_constant__ GemmParams p) {
-    gemm_fwd_body<BLOCK_N, NSPLIT, false>(p);
+    gemm_fwd_body<BLOCK_N, NSPLIT, false, false>(p);
+}
+
+// 16-bit output tiles staged in shared memory and written by TMA stores (GemmParams::out_tma, see make_out_maps).
+template <int BLOCK_N, int NSPLIT>
+__global__ void __launch_bounds__(kThreads, 1) gemm_fwd_tma_kernel(const __grid_constant__ GemmParams p) {
+    gemm_fwd_body<BLOCK_N, NSPLIT, false, true>(p);
 }
 
 // Per-group weights: the class-aware 1x1 output conv and its dgrad, where every crop (4096 rows) reads its class's weight rows.
 template <int BLOCK_N, int NSPLIT>
 __global__ void __launch_bounds__(kThreads, 1) gemm_fwd_grouped_kernel(const __grid_constant__ GemmParams p) {
-    gemm_fwd_body<BLOCK_N, NSPLIT, true>(p);
+    gemm_fwd_body<BLOCK_N, NSPLIT, true, false>(p);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -302,11 +357,13 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_fwd_grouped_kernel(const __g
 template <int BLOCK_N, int NSPLIT, bool GROUPED>
 static int launch_gemm(const GemmParams& p, cudaStream_t stream) {
     using Cfg = GemmCfg<BLOCK_N, NSPLIT>;
-    auto kern = GROUPED ? gemm_fwd_grouped_kernel<BLOCK_N, NSPLIT> : gemm_fwd_kernel<BLOCK_N, NSPLIT>;
-    static bool attr_set = false;
-    if (!attr_set) {
-        GDRN_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
-        attr_set = true;
+    auto kern = GROUPED ? gemm_fwd_grouped_kernel<BLOCK_N, NSPLIT>
+                        : (p.out_tma ? gemm_fwd_tma_kernel<BLOCK_N, NSPLIT> : gemm_fwd_kernel<BLOCK_N, NSPLIT>);
+    static bool attr_set[2] = {false, false};
+    if (!attr_set[p.out_tma]) {
+        GDRN_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                          p.out_tma ? Cfg::SMEM_BYTES_TMA : Cfg::SMEM_BYTES));
+        attr_set[p.out_tma] = true;
     }
     const int groups = (p.nphase ? p.nphase : 1) * p.num_m_tiles * p.num_n_tiles;
     int ctas = groups < num_sms() ? groups : num_sms();
@@ -316,7 +373,7 @@ static int launch_gemm(const GemmParams& p, cudaStream_t stream) {
     memset(&cfg, 0, sizeof(cfg));
     cfg.gridDim = dim3(ctas);
     cfg.blockDim = dim3(kThreads);
-    cfg.dynamicSmemBytes = Cfg::SMEM_BYTES;
+    cfg.dynamicSmemBytes = p.out_tma ? Cfg::SMEM_BYTES_TMA : Cfg::SMEM_BYTES;
     cfg.stream = stream;
     cudaLaunchAttribute attr[1];
     int na = 0;
@@ -360,6 +417,23 @@ static int check_groups(const char* fn, const int* group, int M, int rows_per_gr
                          rows_per_group, kBlockM);
     if (M % rows_per_group != 0) return set_error(GDRN_ERR_ARG, "%s: M=%d is not a whole number of groups of %d rows", fn, M, rows_per_group);
     if (has_bias && bias_stride < 0) return set_error(GDRN_ERR_ARG, "%s: bias_stride=%d must be >= 0", fn, bias_stride);
+    return 0;
+}
+
+// Launches whose 16-bit planes leave through TMA stores (gemm_fwd_tma_kernel): every mode 0 / mode 1 launch with a 16-bit output.
+// Phase-decomposed dgrads (which scatter their rows) and the grouped kernel store directly, and so does a single-pass launch
+// that writes two planes (only one 128-wide plane fits a warpgroup's half of the staging buffer).
+// The output map is [M][min(ldc, N rounded up to 32)]: rows beyond M and the 32-column chunks that start at or beyond N are not
+// written, the columns [N, ldc) of a partial chunk are written as zeros, exactly like the direct stores.
+static int make_out_maps(GemmParams& p, int nsplit) {
+    if (p.out_hi == nullptr || p.group != nullptr || (p.out_lo != nullptr && nsplit == 1)) return 0;
+    const int width = p.ldc < (p.N + 31) / 32 * 32 ? p.ldc : (p.N + 31) / 32 * 32;
+    uint64_t dims[2] = {(uint64_t)width, (uint64_t)p.M};
+    uint64_t strides[1] = {(uint64_t)p.ldc * 2};
+    uint32_t box[2] = {64, 64};
+    if (make_tmap(&p.tmC[0], p.out_hi, 2, dims, strides, box)) return GDRN_ERR_CUDA;
+    if (p.out_lo != nullptr && make_tmap(&p.tmC[1], p.out_lo, 2, dims, strides, box)) return GDRN_ERR_CUDA;
+    p.out_tma = 1;
     return 0;
 }
 
@@ -449,6 +523,7 @@ static int conv_fwd_impl(const void* x_hi, const void* x_lo, const void* w_hi, c
     p.w_group_rows = Cout_pad;
     p.num_w_groups = num_groups;
     p.bias_stride = bias_stride;
+    if (make_out_maps(p, nsplit)) return GDRN_ERR_CUDA;
     return dispatch_gemm(p, block_n, nsplit, stream);
 }
 
@@ -606,6 +681,7 @@ static int gemm_fwd_impl(const void* a_hi, const void* a_lo, const void* w_hi, c
     p.w_group_rows = N_pad;
     p.num_w_groups = num_groups;
     p.bias_stride = bias_stride;
+    if (make_out_maps(p, nsplit)) return GDRN_ERR_CUDA;
     return dispatch_gemm(p, block_n, nsplit, stream);
 }
 

@@ -38,6 +38,10 @@ struct GemmParams {
     // [group[g] * w_group_rows, ...) and bias + group[g] * bias_stride; group[g] is clamped to [0, num_w_groups).
     const int* group;
     int rows_per_group, w_group_rows, num_w_groups, bias_stride;
+    // TMA-stored output (gemm_fwd_tma_kernel, chosen by the host when out_tma is set): the 16-bit planes [plane hi/lo] as
+    // [M][min(ldc, N rounded up to 32)] with {64, 64} boxes
+    int out_tma;
+    CUtensorMap tmC[2];
 };
 
 }  // namespace gdrn

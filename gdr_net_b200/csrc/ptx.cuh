@@ -100,6 +100,31 @@ __device__ __forceinline__ void tma_load_4d_u32(uint32_t dst, uint64_t tmap, uin
         : "memory");
 }
 
+// TMA store of a box from shared memory (swizzled like the tensor map) to global memory; rows / columns outside the map's extent
+// are not written.  Completion is tracked per issuing thread by bulk groups: `bulk_wait_group_read<N>` returns once the shared
+// memory of all but the N most recent groups has been read (the staging buffer may be reused), `bulk_wait_group<N>` once their
+// writes are done.  The generic-proxy writes that fill the box must be made visible with fence_proxy_async() first.
+__device__ __forceinline__ void tma_store_2d_u32(uint64_t tmap, uint32_t src, int c0, int c1) {
+    asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];" ::"l"(tmap), "r"(src), "r"(c0),
+                 "r"(c1)
+                 : "memory");
+}
+__device__ __forceinline__ void bulk_commit_group() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void bulk_wait_group_read() {
+    asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory");
+}
+template <int N>
+__device__ __forceinline__ void bulk_wait_group() {
+    asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory");
+}
+
+// Named barrier `id` (1..15; 0 is __syncthreads) over `threads` threads, a multiple of 32.
+template <int ID, int THREADS>
+__device__ __forceinline__ void named_bar_sync() {
+    asm volatile("bar.sync %0, %1;" ::"n"(ID), "n"(THREADS) : "memory");
+}
+
 __device__ __forceinline__ uint32_t cluster_ctarank() {
     uint32_t r;
     asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
