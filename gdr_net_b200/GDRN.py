@@ -219,8 +219,10 @@ def _check_supported(cfg):
         pose_loss_switches(p)
     except ValueError as e:
         problems.append(str(e))
-    if c.TRANS_HEAD.ENABLED or c.USE_MTL or c.BACKBONE.FREEZE or r.FREEZE or p.FREEZE:
-        problems.append("trans head / MTL weighting / frozen sub-nets (TRANS_HEAD.ENABLED, USE_MTL, FREEZE)")
+    # BACKBONE / ROT_HEAD / PNP_NET .FREEZE are supported in every combination (Engine.live_*); with all three frozen the
+    # optimizer gets no parameters and fails to build, as the reference's does
+    if c.TRANS_HEAD.ENABLED or c.USE_MTL:
+        problems.append("trans head / MTL weighting (TRANS_HEAD.ENABLED, USE_MTL)")
     if problems:
         raise NotImplementedError("gdr_net_b200 implements the a6_cPnP hot path only; unsupported: " + "; ".join(problems))
 
@@ -359,6 +361,16 @@ def _load_backbone_pretrained(backbone, spec: str):
     return missing, unexpected
 
 
+def _freeze_or_add(net, freeze, params_lr_list, lr):
+    """reference GDRN.py:563-571, 595-603, 684-692: a frozen sub-network's parameters stop requiring grad and get no
+    optimizer group; any other one gets a group of its trainable parameters."""
+    if freeze:
+        for p in net.parameters():
+            p.requires_grad_(False)
+    else:
+        params_lr_list.append({"params": [p for p in net.parameters() if p.requires_grad], "lr": lr})
+
+
 def build_model_optimizer(cfg, precision: str = "mixed"):
     """reference GDRN.py:550-724"""
     backbone_cfg = cfg.MODEL.CDPN.BACKBONE
@@ -368,7 +380,7 @@ def build_model_optimizer(cfg, precision: str = "mixed"):
     params_lr_list = []
     _block, layers, channels, _name = resnet_spec[backbone_cfg.NUM_LAYERS]
     backbone_net = ResNetBackboneNet(layers, backbone_cfg.INPUT_CHANNEL, freeze=backbone_cfg.FREEZE)
-    params_lr_list.append({"params": [p for p in backbone_net.parameters() if p.requires_grad], "lr": float(cfg.SOLVER.BASE_LR)})
+    _freeze_or_add(backbone_net, backbone_cfg.FREEZE, params_lr_list, float(cfg.SOLVER.BASE_LR))
 
     r_out_dim, mask_out_dim, region_out_dim = get_xyz_mask_region_out_dim(cfg)
     rot_head_net = RotWithRegionHead(
@@ -378,7 +390,7 @@ def build_model_optimizer(cfg, precision: str = "mixed"):
         num_classes=r_head_cfg.NUM_CLASSES, rot_class_aware=r_head_cfg.ROT_CLASS_AWARE,
         mask_class_aware=r_head_cfg.MASK_CLASS_AWARE, region_class_aware=r_head_cfg.REGION_CLASS_AWARE,
     )
-    params_lr_list.append({"params": [p for p in rot_head_net.parameters() if p.requires_grad], "lr": float(cfg.SOLVER.BASE_LR)})
+    _freeze_or_add(rot_head_net, r_head_cfg.FREEZE, params_lr_list, float(cfg.SOLVER.BASE_LR))
 
     pnp_net_in_channel = r_out_dim
     if pnp_net_cfg.WITH_2D_COORD:
@@ -393,8 +405,7 @@ def build_model_optimizer(cfg, precision: str = "mixed"):
     pnp_head_cfg.update(nIn=pnp_net_in_channel, rot_dim=rot_dim, num_regions=r_head_cfg.NUM_REGIONS, featdim=128,
                         num_layers=3, mask_attention_type=pnp_net_cfg.MASK_ATTENTION)
     pnp_net = ConvPnPNet(**pnp_head_cfg)
-    params_lr_list.append({"params": [p for p in pnp_net.parameters() if p.requires_grad],
-                           "lr": float(cfg.SOLVER.BASE_LR) * pnp_net_cfg.LR_MULT})
+    _freeze_or_add(pnp_net, pnp_net_cfg.FREEZE, params_lr_list, float(cfg.SOLVER.BASE_LR) * pnp_net_cfg.LR_MULT)
 
     model = GDRN(cfg, backbone_net, rot_head_net, trans_head_net=None, pnp_net=pnp_net, precision=precision)
     from .solver import build_optimizer_with_params

@@ -246,6 +246,19 @@ class Engine:
 
         self.pose_sw = PoseSwitches(**sw)
         assert self.pose_ex or self.loss_names == LOSS_NAMES, self.loss_names
+        # frozen sub-networks (BACKBONE / ROT_HEAD / PNP_NET .FREEZE, GDRN.py:550-700): the reference runs a frozen backbone or
+        # head under no_grad and detaches its output, so a frozen head also cuts the backbone off; a frozen Patch-PnP only
+        # stops its own parameters.  live_* = that sub-network's parameters receive gradients; a frozen head's per-pixel
+        # losses are not computed (gdrn_loss, GDRN.py:342-400)
+        cd = model.cfg.MODEL.CDPN
+        self.freeze = (bool(cd.BACKBONE.FREEZE), bool(rh.FREEZE), bool(cd.PNP_NET.FREEZE))
+        self.live_head = not self.freeze[1]
+        self.live_bb = self.live_head and not self.freeze[0]
+        self.live_pnp = not self.freeze[2]
+        self.live_any = self.live_head or self.live_pnp
+        self.n_pix = 5 if self.live_head else 0  # per-pixel losses at the head of the loss vector
+        if not self.live_head:
+            self.loss_names = self.loss_names[5:]
         assert int(C.load().gdrn_pose_loss_count(self.pose_sw)) == len(pose_names), (sw, pose_names)
         self.named_params = list(model.named_parameters())
         self.bn: Dict[str, _BN] = {}
@@ -290,6 +303,14 @@ class Engine:
         from .dist import SEGMENTS, segment_bounds
 
         self._seg = segment_bounds(self.named_params, SEGMENTS)
+        # (parameter, flat_grad offset) of every parameter that can receive a gradient: only these enter _GDRNFunction, so
+        # every other parameter keeps .grad None
+        live = lambda n: self.live_pnp if n.startswith("pnp_net.") else self.live_head if n.startswith("rot_head_net.") else self.live_bb  # noqa: E731
+        self.live_params, off = [], 0
+        for name, p in self.named_params:
+            if live(name):
+                self.live_params.append((p, off))
+            off += p.numel()
 
     def _init_class_tables(self, rows, n_rows):
         """Device tables of the class-aware head: cls_idx [C * cls_npad] = the output-conv row behind each slot of the class-major
@@ -541,15 +562,24 @@ class Engine:
                        region=maps[:, mo + 3:self.n_logits])
         return res
 
+    def _runs_dgrad(self, key: str) -> bool:
+        """Whether backward runs the data gradient of the layer `key` (_conv_modules keys, "deconv", "fc*"): only where a
+        gradient still has to flow to a live parameter below it."""
+        if key.startswith("backbone.") or key == "deconv":
+            return self.live_bb
+        if key.startswith("rot_head_net.") or key == "pnp_net.features.0":
+            return self.live_head
+        return self.live_any  # Patch-PnP convs 3 and 6 and the FC stack
+
     def _prepare_weights_calls(self, need_dgrad: bool):
         m, pl, bpl = self.model, self.planes, self.bplanes
         wf, wd = self.wf, self.wd
         for key, conv in self._conv_modules():
             if key == "rot_head_net.features.23" and self.class_aware:
-                self._class_head_pack_calls(need_dgrad)
+                self._class_head_pack_calls(need_dgrad and self._runs_dgrad(key))
                 continue
             wf[key] = ops.pack_conv_fwd(conv.weight, pl, out=wf.get(key))
-            if need_dgrad:
+            if need_dgrad and self._runs_dgrad(key):
                 # the logit gradient of head_bwd is 128 columns wide whatever the output conv's row count (MO + 4 + R)
                 ipad = 128 if key == "rot_head_net.features.23" else None
                 wd[key] = ops.pack_conv_dgrad(conv.weight, bpl, out=wd.get(key), ipad=ipad)
@@ -557,7 +587,7 @@ class Engine:
         # the ConvTranspose2d forward IS the data gradient of the stride-2 conv whose OIHW weight its IOHW weight is:
         # gdrn_conv_dgrad_s2 evaluates it by output parity over the un-dilated input (no zero-inserted tensor, 1/4 of the MACs)
         wf["deconv"] = ops.pack_conv_dgrad(dc.weight, pl, out=wf.get("deconv"))
-        if need_dgrad:
+        if need_dgrad and self._runs_dgrad("deconv"):
             wd["deconv"] = ops.pack_deconv_dgrad(dc.weight, bpl, out=wd.get("deconv"))
         pn = m.pnp_net
         wf["fc1"] = ops.pack_linear(pn.fc1.weight, pl, out=wf.get("fc1"), nhwc_from=(128, 8, 8))
@@ -566,7 +596,7 @@ class Engine:
             self.w_rt = torch.empty(pn.fc_r.out_features + 3, pn.fc_r.in_features, device=self.dev)
             self.b_rt = torch.empty(pn.fc_r.out_features + 3, device=self.dev)
         wf["fc_rt"] = ops.pack_linear(self.w_rt, pl, out=wf.get("fc_rt"))
-        if need_dgrad:
+        if need_dgrad and self._runs_dgrad("fc_rt"):
             wd["fc1"] = ops.pack_linear(pn.fc1.weight, bpl, out=wd.get("fc1"), nhwc_from=(128, 8, 8), transpose=True)
             wd["fc2"] = ops.pack_linear(pn.fc2.weight, bpl, out=wd.get("fc2"), transpose=True)
             wd["fc_rt"] = ops.pack_linear(self.w_rt, bpl, out=wd.get("fc_rt"), transpose=True)
@@ -666,8 +696,12 @@ class Engine:
                         return self._eval_graphed(x, aux, want_maps)
                     return self.forward_eval_folded(x, aux, want_maps=want_maps)
                 return self.forward(x, aux, train_bn=train_bn, do_loss=False, want_maps=want_maps)
-        params = [p for _, p in self.named_params]
-        losses, vis = _GDRNFunction.apply(self, x, aux, train_bn, *params)
+        if not self.live_any:  # frozen head and Patch-PnP: nothing to differentiate, the losses do not require grad
+            with torch.no_grad():
+                res = self.forward(x, aux, train_bn=train_bn, do_loss=True)
+            self.saved = None
+            return dict(losses=res["losses"], vis=res["vis"])
+        losses, vis = _GDRNFunction.apply(self, x, aux, train_bn, *[p for p, _ in self.live_params])
         return dict(losses=losses, vis=vis)
 
     def forward(self, x: torch.Tensor, aux: dict, train_bn: bool, do_loss: bool, want_maps: bool = False) -> dict:
@@ -681,7 +715,9 @@ class Engine:
         if train_bn:
             (self.stats_all if self.deterministic else self.stats64_all).zero_()
         S = dict(B=B, train_bn=train_bn) if do_loss else None
-        self._want_masks = do_loss
+        # a sub-network nothing differentiates through (frozen, or below a frozen head) runs the non-saving path of inference
+        keep_bb, keep_head = do_loss and self.live_bb, do_loss and self.live_head
+        self._want_masks = keep_bb
 
         # ---- a1: backbone (resnet_backbone.py:69-76)
         a_col = PT((B * 128 * 128, 192), pl, device=dev)
@@ -690,7 +726,7 @@ class Engine:
         st0 = self.bn["backbone.bn1"]
         u0 = ops.gemm_fwd(a_col, self.wf["stem"], 64, stats=st0.stats64 if (train_bn and not self.deterministic) else None).view(B, 128, 128, 64)
         a0 = self._bn_fwd("backbone.bn1", u0, True, train_bn)
-        if S is not None:
+        if keep_bb:
             cur, pool_arg = ops.maxpool_fwd(a0, want_arg=True)
             S["stem"] = dict(a_col=a_col, u0=u0, a0=a0, pool_arg=pool_arg, m0=self._last_mask)
             S["blocks"] = []
@@ -707,15 +743,16 @@ class Engine:
                 else:
                     idn = cur
                 u2, out = self._conv_bn(a1, p + ".conv2", blk.conv2, p + ".bn2", True, train_bn, res=idn)
-                if S is not None:
+                if keep_bb:
                     S["blocks"].append(dict(p=p, blk=blk, x_in=cur, u1=u1, a1=a1, u2=u2, out=out, ud=ud, m1=m1, m2=self._last_mask))
                 cur = out
         feat = cur  # [B,8,8,512]
 
         # ---- a2: geometry head (cdpn_rot_head_region.py:80-135)
         hf = m.rot_head_net.features
+        self._want_masks = keep_head
         u, y = self._conv_bn(feat, "deconv", hf[0], "rot_head_net.features.1", True, train_bn)
-        if S is not None:
+        if keep_head:
             S["deconv"] = dict(z=feat, u=u, y=y, m=self._last_mask)
             S["head"] = []
         cur = y
@@ -723,7 +760,7 @@ class Engine:
             if up:
                 cur = ops.upsample2x_fwd(cur)
             u, y = self._conv_bn(cur, f"rot_head_net.features.{ci}", hf[ci], f"rot_head_net.features.{bi}", True, train_bn)
-            if S is not None:
+            if keep_head:
                 S["head"].append(dict(ci=ci, bi=bi, up=up, x_in=cur, u=u, y=y, m=self._last_mask))
             cur = y
         head_in = cur  # [B,64,64,256]
@@ -737,21 +774,24 @@ class Engine:
         logits, pnp_in, pred, (flat, h1, h2) = self._head_pnp(head_in, aux, pnp_saved)
 
         # ---- a5/a6 pose decode + a7..a10 losses
-        pix_sums = torch.empty(7, dtype=torch.float64, device=dev)
-        m_xyz, m_mask, m_region = self._loss_masks(aux)
-        pix = (logits.data_ptr(), aux["gt_xyz"].data_ptr(), m_xyz, m_mask, m_region, aux["gt_region"].data_ptr(), pix_sums.data_ptr(), B,
-               4096, self.mask_loss, self.mask_out)
-        if self.regions_ex2:
-            C.gdrn_pixel_loss_fwd_ex2(*pix, self.num_regions, self.region_att, self.pnp_ld, _stream())
-        else:
-            C.gdrn_pixel_loss_fwd_ex(*pix, _stream())
-        S.update(logits=logits, pnp_in=pnp_in, pnp=pnp_saved, flat=flat, h1=h1, h2=h2, pred=pred, head_in=head_in,
+        if self.live_head:
+            pix_sums = torch.empty(7, dtype=torch.float64, device=dev)
+            m_xyz, m_mask, m_region = self._loss_masks(aux)
+            pix = (logits.data_ptr(), aux["gt_xyz"].data_ptr(), m_xyz, m_mask, m_region, aux["gt_region"].data_ptr(), pix_sums.data_ptr(),
+                   B, 4096, self.mask_loss, self.mask_out)
+            if self.regions_ex2:
+                C.gdrn_pixel_loss_fwd_ex2(*pix, self.num_regions, self.region_att, self.pnp_ld, _stream())
+            else:
+                C.gdrn_pixel_loss_fwd_ex(*pix, _stream())
+        else:  # frozen head: no per-pixel losses; the finalize kernel's first five outputs are dropped below
+            pix_sums = torch.zeros(7, dtype=torch.float64, device=dev)
+        S.update(logits=logits, pnp_in=pnp_in, pnp=pnp_saved, flat=flat, h1=h1, h2=h2, pred=pred, head_in=head_in if keep_head else None,
                  pix_sums=pix_sums, aux=aux)
         self.saved = S
         # the pose kernel needs the upstream loss gradients to emit dY9; forward calls it with unit weights and
         # backward re-runs it (cheap: B CTAs) with the actual ones.
         self._pose(S, gw=None)
-        losses = torch.empty(len(self.loss_names), device=dev)
+        losses = torch.empty(5 - self.n_pix + len(self.loss_names), device=dev)  # the five per-pixel slots always
         vis2 = torch.empty(2, device=dev)
         n_pts = aux["gt_points"].shape[1]
         if self.pose_ex:
@@ -761,6 +801,8 @@ class Engine:
             C.gdrn_loss_finalize_ex(pix_sums.data_ptr(), S["pose_sums"].data_ptr(), S["vis_ps"].data_ptr(), losses.data_ptr(),
                                     vis2.data_ptr(), B, 4096, n_pts, _stream())
         vis = torch.cat([vis2, S["out_trans"][0], pred[0, 6:9], aux["gt_trans"][0], aux["gt_trans_ratio"][0]])
+        if not self.live_head:
+            losses = losses[5:]
         return dict(rot=S["out_rot"], trans=S["out_trans"], pred=pred, losses=losses, vis=vis, logits=logits)
 
     def _loss_masks(self, aux) -> tuple:
@@ -790,7 +832,7 @@ class Engine:
             sym_idx = aux["sym_idx"] = self.sym_table.indices(aux["sym_infos"])
         syms = self.sym_table.table if sym_idx is not None else None
         if gw is None:
-            gw = torch.ones(len(self.loss_names) - 5, device=dev)
+            gw = torch.ones(len(self.loss_names) - self.n_pix, device=dev)
         n_pts = aux["gt_points"].shape[1]
         if self.pose_ex:
             C.gdrn_pose_loss_ex(S["pred"].data_ptr(), 16, aux["roi_cams"].data_ptr(), aux["roi_centers"].data_ptr(),
@@ -859,6 +901,8 @@ class Engine:
         self.flat_grad)."""
         S, m, dev = self.saved, self.model, self.dev
         assert S is not None, "backward called without a do_loss forward"
+        if not self.live_any:  # frozen head and Patch-PnP: no parameter receives a gradient
+            return self._backward_done()
         B, aux, pn = S["B"], S["aux"], m.pnp_net
         bp = self.bplanes
 
@@ -870,39 +914,50 @@ class Engine:
         gw = grad_losses.float().contiguous()
         if self.grad_scale != 1.0:
             gw = gw * self.grad_scale  # the whole backward is linear in the loss gradients
-        self._pose(S, gw=gw[5:].contiguous())
+        self._pose(S, gw=gw[self.n_pix:].contiguous())
         dy9 = S["dy9"]
         tmp = torch.empty(1024, device=dev)
+        wg = self.live_pnp  # a frozen Patch-PnP passes the gradient through but computes no weight or bias gradient
 
         # ---- FC stack (conv_pnp_net.py:152-156)
-        buf, ks, kss = ops.gemm_wgrad(dy9, h(S["h2"]), self.ws)
-        ops.unpack_wgrad(buf, self.grads["pnp_net.fc_r.weight"], 6, 256, 1, 1, 256, ks, kss, 256, 1, 0, 0)
-        ops.unpack_wgrad(buf[6 * 256:], self.grads["pnp_net.fc_t.weight"], 3, 256, 1, 1, 256, ks, kss, 256, 1, 0, 0)
-        C.gdrn_colsum(dy9.hi_ptr, dy9.lo_ptr, tmp.data_ptr(), B, 64, _stream())
-        self.grads["pnp_net.fc_r.bias"].copy_(tmp[0:6])
-        self.grads["pnp_net.fc_t.bias"].copy_(tmp[6:9])
+        if wg:
+            buf, ks, kss = ops.gemm_wgrad(dy9, h(S["h2"]), self.ws)
+            ops.unpack_wgrad(buf, self.grads["pnp_net.fc_r.weight"], 6, 256, 1, 1, 256, ks, kss, 256, 1, 0, 0)
+            ops.unpack_wgrad(buf[6 * 256:], self.grads["pnp_net.fc_t.weight"], 3, 256, 1, 1, 256, ks, kss, 256, 1, 0, 0)
+            C.gdrn_colsum(dy9.hi_ptr, dy9.lo_ptr, tmp.data_ptr(), B, 64, _stream())
+            self.grads["pnp_net.fc_r.bias"].copy_(tmp[0:6])
+            self.grads["pnp_net.fc_t.bias"].copy_(tmp[6:9])
         dh2 = ops.gemm_fwd(dy9, self.wd["fc_rt"], 256)
         dz2 = self._leaky_bwd(dh2, h(S["h2"]))
-        buf, ks, kss = ops.gemm_wgrad(dz2, h(S["h1"]), self.ws)
-        ops.unpack_wgrad(buf, self.grads["pnp_net.fc2.weight"], 256, 1024, 1, 1, 1024, ks, kss, 1024, 1, 0, 0)
-        C.gdrn_colsum(dz2.hi_ptr, dz2.lo_ptr, self.grads["pnp_net.fc2.bias"].data_ptr(), B, 256, _stream())
+        if wg:
+            buf, ks, kss = ops.gemm_wgrad(dz2, h(S["h1"]), self.ws)
+            ops.unpack_wgrad(buf, self.grads["pnp_net.fc2.weight"], 256, 1024, 1, 1, 1024, ks, kss, 1024, 1, 0, 0)
+            C.gdrn_colsum(dz2.hi_ptr, dz2.lo_ptr, self.grads["pnp_net.fc2.bias"].data_ptr(), B, 256, _stream())
         dh1 = ops.gemm_fwd(dz2, self.wd["fc2"], 1024)
         dz1 = self._leaky_bwd(dh1, h(S["h1"]))
-        buf, ks, kss = ops.gemm_wgrad(dz1, h(S["flat"]), self.ws)
-        ops.unpack_wgrad(buf, self.grads["pnp_net.fc1.weight"], 1024, 128, 8, 8, 128, ks, kss, 8192, 64, 8, 1)
-        C.gdrn_colsum(dz1.hi_ptr, dz1.lo_ptr, self.grads["pnp_net.fc1.bias"].data_ptr(), B, 1024, _stream())
+        if wg:
+            buf, ks, kss = ops.gemm_wgrad(dz1, h(S["flat"]), self.ws)
+            ops.unpack_wgrad(buf, self.grads["pnp_net.fc1.weight"], 1024, 128, 8, 8, 128, ks, kss, 8192, 64, 8, 1)
+            C.gdrn_colsum(dz1.hi_ptr, dz1.lo_ptr, self.grads["pnp_net.fc1.bias"].data_ptr(), B, 1024, _stream())
         g = ops.gemm_fwd(dz1, self.wd["fc1"], 8192).view(B, 8, 8, 128)
 
         # ---- Patch-PnP convs (conv_pnp_net.py:76-80)
         pf = pn.features
         for L in reversed(S["pnp"]):
             ci, gi = L["ci"], L["gi"]
+            # a frozen Patch-PnP's GroupNorm parameter sums land in its slice of flat_grad, which is never read
             du = ops.gn_relu_bwd(g, h(L["y"]), h(L["u"]), pf[gi].weight, L["gstats"], self.grads[f"pnp_net.features.{gi}.weight"],
                                  self.grads[f"pnp_net.features.{gi}.bias"], G=pf[gi].num_groups)
-            self._wgrad_conv(du, h(L["x_in"]), pf[ci], f"pnp_net.features.{ci}.weight")
+            if wg:
+                self._wgrad_conv(du, h(L["x_in"]), pf[ci], f"pnp_net.features.{ci}.weight")
+            if ci == 0 and not self.live_head:  # a frozen head needs no Patch-PnP input gradient
+                break
             g = self._dgrad_conv(du, pf[ci], f"pnp_net.features.{ci}")
+        if wg:
+            self._segment_done("pnp_net")
+        if not self.live_head:
+            return self._backward_done()
         d_pnp_in = g  # [B,64,64,pnp_ld]
-        self._segment_done("pnp_net")
 
         # ---- glue + per-pixel losses backward (one fused pass over the logits)
         dlog = PT((B * 4096, 128), bp, device=dev)
@@ -947,6 +1002,9 @@ class Engine:
             ops.unpack_wgrad(buf, self.grads["rot_head_net.features.0.weight"], 512, 256, 3, 3, 256, ks, kss, 256 * 9, 9, 3, 1)
 
         self._on_side(deconv_wgrad, keep=(du,))
+        if not self.live_bb:  # frozen backbone: the head's gradients end the step
+            self._segment_done("rot_head_net")
+            return self._backward_done()
         g = ops.conv_fwd(du, self.wd["deconv"], 512, 3, 3, 2, 1)  # [B,8,8,512]
         self._segment_done("rot_head_net")
 
@@ -980,6 +1038,12 @@ class Engine:
 
         self._on_side(stem_wgrad, keep=(du0,))
         self._segment_done("backbone.stem")  # layer1 + bn1 + conv1 (joins the wgrad side stream)
+        self.saved = None
+        return self.grads
+
+    def _backward_done(self):
+        """End of a backward that stops above the backbone: join the side stream (a no-op after _segment_done) and free S."""
+        self._join_side()
         self.saved = None
         return self.grads
 
@@ -1197,10 +1261,8 @@ class _GDRNFunction(torch.autograd.Function):
         _finish_hook(engine)  # the gradients handed to autograd are the all-reduced ones (stream-ordered wait, no host sync)
         # FRESH views of the flat gradient buffer: autograd's AccumulateGrad adopts a uniquely-referenced contiguous gradient
         # without copying, so after `zero_grad(set_to_none=True)` p.grad aliases Engine.flat_grad and the 148 per-parameter
-        # clone kernels (0.4 ms per step) disappear.  materialize_aliased_grads() protects gradient accumulation.
-        flat, outs, off = engine.flat_grad, [], 0
-        for _, p in engine.named_params:
-            n = p.numel()
-            outs.append(flat[off:off + n].view_as(p))
-            off += n
+        # clone kernels (0.4 ms per step) disappear.  materialize_aliased_grads() protects gradient accumulation.  Only the
+        # live parameters are inputs of the function (Engine.live_params): frozen and unreachable ones keep .grad None.
+        flat = engine.flat_grad
+        outs = [flat[off:off + p.numel()].view_as(p) for p, off in engine.live_params]
         return (None, None, None, None) + tuple(outs)
