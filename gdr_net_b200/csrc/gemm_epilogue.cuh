@@ -22,6 +22,8 @@ namespace gdrn {
 //          stg + p * (J1 - J0) * 1024: one 128-byte-swizzled [64 rows][64 columns] box per 64 columns, 8 KB apart), from where
 //          the kernel stores them with TMA.  fp32 outputs are always stored here.
 // J0, J1 : the column groups (8 columns each) of this call; a 128-wide 3-pass tile is staged in two 64-column halves.
+// PLAIN  : bias and activation only, one 16-bit plane (the 256-row tile): the residual, lo-plane, fp32-output, statistics and
+//          output-parity code is not compiled in.
 // Staging slot of (column group j, row half h) of this thread's first plane: row r of a box keeps its 16-byte column chunk c at
 // chunk c ^ (r % 8) (SWIZZLE_128B); the 8 rows of a warp's store have distinct r % 8, so the 32 lanes hit 32 distinct banks.
 __device__ __forceinline__ uint32_t* stage_slot(uint8_t* stg, int row0, int lane, int j, int h) {
@@ -29,13 +31,15 @@ __device__ __forceinline__ uint32_t* stage_slot(uint8_t* stg, int row0, int lane
                                        h * 1024);
 }
 
-template <int BLOCK_N, bool GROUPED = false, bool STAGED = false, int J0 = 0, int J1 = BLOCK_N / 8>
+template <int BLOCK_N, bool GROUPED = false, bool STAGED = false, int J0 = 0, int J1 = BLOCK_N / 8, bool PLAIN = false>
 __device__ __forceinline__ void gemm_epilogue_tile(const GemmParams& p, const float* acc, int lane, int row0, int m_tile, int n_tile,
                                                    int ph, float* s_stats, int bias_off = 0, uint8_t* stg = nullptr) {
+    static_assert(!PLAIN || STAGED, "the plain epilogue is the TMA-stored one");
     __nv_bfloat16* out_hi = reinterpret_cast<__nv_bfloat16*>(p.out_hi);
-    __nv_bfloat16* out_lo = reinterpret_cast<__nv_bfloat16*>(p.out_lo);
-    const __nv_bfloat16* res_hi = reinterpret_cast<const __nv_bfloat16*>(p.res_hi);
-    const __nv_bfloat16* res_lo = reinterpret_cast<const __nv_bfloat16*>(p.res_lo);
+    __nv_bfloat16* out_lo = PLAIN ? nullptr : reinterpret_cast<__nv_bfloat16*>(p.out_lo);
+    const __nv_bfloat16* res_hi = PLAIN ? nullptr : reinterpret_cast<const __nv_bfloat16*>(p.res_hi);
+    const __nv_bfloat16* res_lo = PLAIN ? nullptr : reinterpret_cast<const __nv_bfloat16*>(p.res_lo);
+    float* const out_f32 = PLAIN ? nullptr : p.out_f32;
     const int q = lane & 3;
     uint32_t off[2];  // element offset of (output row, this thread's first column) in the [rows][ldc] planes
     bool row_ok[2];
@@ -44,7 +48,7 @@ __device__ __forceinline__ void gemm_epilogue_tile(const GemmParams& p, const fl
         const int mrow = m_tile * 128 + row0 + 8 * h;
         row_ok[h] = mrow < p.M;
         uint32_t grow = (uint32_t)mrow;  // output row
-        if (p.nphase) {  // (n, i, j) of the dY lattice -> pixel (2i + a, 2j + b) of the 2x larger dX
+        if (!PLAIN && p.nphase) {  // (n, i, j) of the dY lattice -> pixel (2i + a, 2j + b) of the 2x larger dX
             const uint32_t j = grow & ((1u << p.pw_log2) - 1);
             const uint32_t t = grow >> p.pw_log2;
             const uint32_t i = t & ((1u << p.ph_log2) - 1);
@@ -119,7 +123,7 @@ __device__ __forceinline__ void gemm_epilogue_tile(const GemmParams& p, const fl
                 if (!row_ok[h]) continue;
                 const float a = ok0 ? f[h][0] : 0.f, b = ok1 ? f[h][1] : 0.f;
                 const uint32_t o = off[h] + 8 * j;
-                if (p.out_f32 != nullptr) *reinterpret_cast<float2*>(p.out_f32 + o) = make_float2(a, b);
+                if (out_f32 != nullptr) *reinterpret_cast<float2*>(out_f32 + o) = make_float2(a, b);
                 if (!STAGED && out_hi != nullptr) {
                     uint32_t hi, lo;
                     if (out_lo != nullptr) {
@@ -132,7 +136,7 @@ __device__ __forceinline__ void gemm_epilogue_tile(const GemmParams& p, const fl
                 }
             }
         }
-        if (p.stats != nullptr) {
+        if (!PLAIN && p.stats != nullptr) {
             // per-channel sum / sum of squares over the warp's 16 rows: the 8 lanes sharing q hold the same two columns
             float s1[2], s2[2];
 #pragma unroll

@@ -19,6 +19,7 @@
 //     warpgroups run a tile's epilogue the producer already fills the stages of the next tile.  gemm_fwd_tma_kernel (every
 //     launch with a 16-bit output but the phase dgrads, make_out_maps) instead stages the 16-bit planes in a shared-memory buffer
 //     behind the ring and writes them with TMA stores, so the MMAs of the next tile start while the tile drains.
+//     gemm_fwd_tall_kernel (large single-pass launches with a plain epilogue, pick_block_m) runs the same body on 256-row tiles.
 //     Warp 8 = TMA producer.  With nine warps ptxas allots at most 168 registers per thread (three warps share one SM
 //     sub-partition's register file).  A 128-wide 3-pass tile holds 128 accumulator registers (main + cross) in its main
 //     loop; it fits (ptxas -v: 162 registers, no spills) because the cross accumulator is folded into the main one before
@@ -43,10 +44,14 @@ constexpr int kSmemBudget = 227 * 1024;
 constexpr int kAuxBytes = 4096;  // barriers + [2][BLOCK_N] BatchNorm partial sums
 constexpr int kThreads = 288;    // two MMA warpgroups + one producer warp
 
-template <int BLOCK_N, int NSPLIT>
+// BLOCK_M = 256 (gemm_fwd_tall_kernel): every MMA warpgroup owns 128 rows as two 64-row halves, and the A tile is two
+// 128-row TMA boxes.  A single-pass k-block then moves 48 KB of operands for 4.2 MFLOP (85 FLOP per byte) instead of 32 KB for
+// 2.1 MFLOP (64 FLOP per byte): the single-pass 128 x 128 tile is bound by the L2 -> SM operand traffic, not by the MMAs.
+template <int BLOCK_N, int NSPLIT, int BLOCK_M = kBlockM>
 struct GemmCfg {
     static constexpr int NPL = (NSPLIT == 1) ? 1 : 2;
-    static constexpr int A_BYTES = kBlockM * kBlockK * 2;
+    static constexpr int MH = BLOCK_M / kBlockM;  // 64-row MMA halves per warpgroup and 128-row A boxes per stage
+    static constexpr int A_BYTES = BLOCK_M * kBlockK * 2;
     static constexpr int B_BYTES = BLOCK_N * kBlockK * 2;
     static constexpr int STAGE_BYTES = NPL * (A_BYTES + B_BYTES);
     static constexpr int STAGES_RAW = (kSmemBudget - kAuxBytes - 1024) / STAGE_BYTES;
@@ -54,7 +59,7 @@ struct GemmCfg {
     static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + kAuxBytes + 1024;
     // gemm_fwd_tma_kernel: a 32 KB output staging buffer behind the ring (16 KB per MMA warpgroup: its 64 rows of one 128-wide or
     // two 64-wide 16-bit planes), paid for by a smaller aux area (barriers at +0, the [2][BLOCK_N] partial sums at +512); the ring
-    // keeps its stages.
+    // keeps its stages.  The 256-row tile has 4 stages of 48 KB: 192 KB + 32 KB + 3 KB = 227 KB.
     static constexpr int OUT_STAGE_BYTES = 32768;
     static constexpr int SMEM_BYTES_TMA = STAGES * STAGE_BYTES + OUT_STAGE_BYTES + 2048 + 1024;
     static_assert(SMEM_BYTES_TMA <= kSmemBudget, "no room for the output staging buffer");
@@ -65,8 +70,9 @@ struct GemmCfg {
     // a_hi once less, but an MMA that writes part of the registers of one still in flight makes ptxas serialise the whole
     // wgmma chain (warning C7511); the three-MMA form measured 0.9 % faster per step.
     static constexpr int NACC = (NSPLIT == 3) ? 2 : 1;
-    static constexpr int ACC_REGS = NACC * BLOCK_N / 2;  // per thread: 64 rows x NACC * BLOCK_N columns over 128 threads
+    static constexpr int ACC_REGS = NACC * BLOCK_N / 2;  // per thread and 64-row half: 64 rows x NACC * BLOCK_N columns / 128 threads
     static_assert(STAGES >= 2, "pipeline too shallow");
+    static_assert(MH == 1 || (MH == 2 && NSPLIT == 1), "256-row tiles are single-pass only (128 accumulator registers)");
 };
 
 // Weight group of an M-tile (GROUPED): tiles never straddle a group (the entry points require rows_per_group % 128 == 0), and
@@ -76,11 +82,17 @@ __device__ __forceinline__ int tile_group(const GemmParams& p, int m_tile) {
     return min(max(g, 0), p.num_w_groups - 1);
 }
 
-template <int BLOCK_N, int NSPLIT, bool GROUPED, bool OUT_TMA>
+// BLOCK_M = 256 only with OUT_TMA and a plain epilogue (pick_block_m): bias and activation, one 16-bit output plane; no residual,
+// fp32 output, BatchNorm statistics or output-parity phases, so the tall kernel does not carry their code.
+template <int BLOCK_N, int NSPLIT, bool GROUPED, bool OUT_TMA, int BLOCK_M = kBlockM>
 __device__ __forceinline__ void gemm_fwd_body(const GemmParams& p) {
-    using Cfg = GemmCfg<BLOCK_N, NSPLIT>;
+    using Cfg = GemmCfg<BLOCK_N, NSPLIT, BLOCK_M>;
     constexpr int NPL = Cfg::NPL;
     constexpr int STAGES = Cfg::STAGES;
+    constexpr int MH = Cfg::MH;
+    constexpr bool PLAIN = MH == 2;
+    static_assert(!PLAIN || (OUT_TMA && !GROUPED), "the 256-row tile stores with TMA");
+    constexpr int BOX_BYTES = kBlockM * kBlockK * 2;  // one 128-row A box
 
     // 1024-byte alignment by POINTER arithmetic on the __shared__ array (not through uintptr_t): the compiler keeps the
     // shared address space, so the epilogue's statistics compile to shared-memory atomics instead of generic ones
@@ -138,12 +150,17 @@ __device__ __forceinline__ void gemm_fwd_body(const GemmParams& p) {
             const int m_tile = rem / p.num_n_tiles;
             const int bn0 = n_tile * BLOCK_N + (GROUPED ? tile_group(p, m_tile) * p.w_group_rows : 0);
             if (mode == 1) {
-                int n0 = 0, h0 = 0;
-                if (p.TN == 1) {
-                    n0 = m_tile / p.tiles_per_img;
-                    h0 = (m_tile - n0 * p.tiles_per_img) * p.TH;
-                } else {
-                    n0 = m_tile * p.TN;
+                int n0[MH], h0[MH];  // image and first output row of each 128-row box of the tile
+#pragma unroll
+                for (int b = 0; b < MH; ++b) {
+                    const int t = m_tile * MH + b;
+                    if (p.TN == 1) {
+                        n0[b] = t / p.tiles_per_img;
+                        h0[b] = (t - n0[b] * p.tiles_per_img) * p.TH;
+                    } else {
+                        n0[b] = t * p.TN;
+                        h0[b] = 0;
+                    }
                 }
                 int r = 0, s2 = 0;
                 for (int t = 0; t < ntap; ++t) {
@@ -167,15 +184,17 @@ __device__ __forceinline__ void gemm_fwd_body(const GemmParams& p) {
                     }
                     const uint64_t tmA0 = reinterpret_cast<uint64_t>(&p.tmA[0][map]);
                     const uint64_t tmA1 = reinterpret_cast<uint64_t>(&p.tmA[1][map]);
-                    const int hh = h0 + dh;
                     int kw = wt * cch * kBlockK;
                     for (int cc = 0; cc < cch; ++cc, kw += kBlockK) {
                         const uint32_t fb = full0 + stage * 8, dst = smem_base + stage * Cfg::STAGE_BYTES;
                         mbar_wait_u32(empty0 + stage * 8, phase ^ 1);
                         if (elect_one()) {
                             mbar_arrive_expect_tx_u32(fb, Cfg::STAGE_BYTES);
-                            tma_load_4d_u32(dst, tmA0, fb, cc * kBlockK, dw, hh, n0);
-                            if (NPL == 2) tma_load_4d_u32(dst + Cfg::A_BYTES, tmA1, fb, cc * kBlockK, dw, hh, n0);
+#pragma unroll
+                            for (int b = 0; b < MH; ++b) {
+                                tma_load_4d_u32(dst + b * BOX_BYTES, tmA0, fb, cc * kBlockK, dw, h0[b] + dh, n0[b]);
+                                if (NPL == 2) tma_load_4d_u32(dst + Cfg::A_BYTES + b * BOX_BYTES, tmA1, fb, cc * kBlockK, dw, h0[b] + dh, n0[b]);
+                            }
                             tma_load_2d_u32(dst + NPL * Cfg::A_BYTES, tmB0, fb, kw, bn0);
                             if (NPL == 2) tma_load_2d_u32(dst + NPL * Cfg::A_BYTES + Cfg::B_BYTES, tmB1, fb, kw, bn0);
                         }
@@ -189,14 +208,17 @@ __device__ __forceinline__ void gemm_fwd_body(const GemmParams& p) {
             } else {
                 const uint64_t tmA0 = reinterpret_cast<uint64_t>(&p.tmA[0][0]);
                 const uint64_t tmA1 = reinterpret_cast<uint64_t>(&p.tmA[1][0]);
-                const int row0 = m_tile * kBlockM;
+                const int row0 = m_tile * BLOCK_M;
                 for (int kb = 0, kc = 0; kb < p.num_kb; ++kb, kc += kBlockK) {
                     const uint32_t fb = full0 + stage * 8, dst = smem_base + stage * Cfg::STAGE_BYTES;
                     mbar_wait_u32(empty0 + stage * 8, phase ^ 1);
                     if (elect_one()) {
                         mbar_arrive_expect_tx_u32(fb, Cfg::STAGE_BYTES);
-                        tma_load_2d_u32(dst, tmA0, fb, kc, row0);
-                        if (NPL == 2) tma_load_2d_u32(dst + Cfg::A_BYTES, tmA1, fb, kc, row0);
+#pragma unroll
+                        for (int b = 0; b < MH; ++b) {
+                            tma_load_2d_u32(dst + b * BOX_BYTES, tmA0, fb, kc, row0 + b * kBlockM);
+                            if (NPL == 2) tma_load_2d_u32(dst + Cfg::A_BYTES + b * BOX_BYTES, tmA1, fb, kc, row0 + b * kBlockM);
+                        }
                         tma_load_2d_u32(dst + NPL * Cfg::A_BYTES, tmB0, fb, kc, bn0);
                         if (NPL == 2) tma_load_2d_u32(dst + NPL * Cfg::A_BYTES + Cfg::B_BYTES, tmB1, fb, kc, bn0);
                     }
@@ -212,7 +234,7 @@ __device__ __forceinline__ void gemm_fwd_body(const GemmParams& p) {
     }
 
     // ---------------------------------------------------------------------- MMA + epilogue warpgroups
-    const int cw = wg;  // rows [64 cw, 64 cw + 64) of every tile
+    const int cw = wg;  // rows [64 cw, 64 cw + 64) of every tile; of a 256-row tile rows [128 cw, 128 cw + 128)
     const uint64_t desc_const = make_wgmma_desc(0, 16, 1024);
     const uint32_t smem_base = smem_u32(smem), full0 = smem_u32(full_bar), empty0 = smem_u32(empty_bar);
     const bool signaller = (threadIdx.x & 127) == 0;
@@ -240,11 +262,11 @@ __device__ __forceinline__ void gemm_fwd_body(const GemmParams& p) {
         }
         const int n_tile = rem % p.num_n_tiles;
         const int m_tile = rem / p.num_n_tiles;
-        float acc[Cfg::ACC_REGS];
+        float acc[MH * Cfg::ACC_REGS];  // [64-row half][ACC_REGS]
         int prev_stage = -1;
         for (int kb = 0; kb < nkb; ++kb) {
             const uint32_t a_addr = smem_base + stage * Cfg::STAGE_BYTES;
-            const uint64_t da = desc_const | (uint64_t)((a_addr + cw * (64 * 128)) >> 4);
+            const uint64_t da = desc_const | (uint64_t)((a_addr + cw * MH * (64 * 128)) >> 4);
             const uint64_t db = desc_const | (uint64_t)((a_addr + NPL * Cfg::A_BYTES) >> 4);
             mbar_wait_u32(full0 + stage * 8, phase);
             wgmma_fence_regs(acc);
@@ -257,7 +279,9 @@ __device__ __forceinline__ void gemm_fwd_body(const GemmParams& p) {
                     Wgmma<BLOCK_N, 0, 0>::mma(acc + BLOCK_N / 2, da + 2 * k, db + (Cfg::B_BYTES >> 4) + 2 * k, ac);  // a_hi x w_lo -> cross
                     Wgmma<BLOCK_N, 0, 0>::mma(acc + BLOCK_N / 2, da + (Cfg::A_BYTES >> 4) + 2 * k, db + 2 * k, 1u);  // a_lo x w_hi -> cross
                 } else {
-                    Wgmma<BLOCK_N, 0, 0>::mma(acc, da + 2 * k, db + 2 * k, ac);
+#pragma unroll
+                    for (int h = 0; h < MH; ++h)  // 64-row half h: A rows 64 h further on, (64 * 128) >> 4 descriptor units
+                        Wgmma<BLOCK_N, 0, 0>::mma(acc + h * Cfg::ACC_REGS, da + h * 512 + 2 * k, db + 2 * k, ac);
                 }
             }
             wgmma_commit();
@@ -286,37 +310,49 @@ __device__ __forceinline__ void gemm_fwd_body(const GemmParams& p) {
         if constexpr (GROUPED) {
             gemm_epilogue_tile<BLOCK_N, true>(p, acc, lane, row0, m_tile, n_tile, ph, s_stats, tile_group(p, m_tile) * p.bias_stride);
         } else if constexpr (OUT_TMA) {
-            const int grow0 = m_tile * kBlockM + cw * 64;  // first output row of this warpgroup
-            auto store = [&](int box0) {                   // one thread: the staged boxes of both planes
-                if (grow0 < p.M) {
+            // the 128-row tile holding this warpgroup's rows, and the row of it in acc[4j + 0..1] of the first 64-row half
+            const int m128 = MH == 2 ? 2 * m_tile + cw : m_tile;
+            const int r0 = MH == 2 ? row0 - cw * 64 : row0;
+            const int grow0 = m128 * kBlockM + r0 - (r0 & 63);  // first output row of this warpgroup('s first half)
+            auto store = [&](int first_row, int box0) {       // one thread: the staged boxes of both planes
+                if (first_row < p.M) {
                     for (int pl = 0; pl < (p.out_lo != nullptr ? 2 : 1); ++pl)
                         for (int b = 0; b < JP / 8; ++b)
                             if (n_tile * BLOCK_N + 64 * (box0 + b) < p.N)
                                 tma_store_2d_u32(reinterpret_cast<uint64_t>(&p.tmC[pl]), smem_u32(stg) + (pl * (JP / 8) + b) * 8192,
-                                                 n_tile * BLOCK_N + 64 * (box0 + b), grow0);
+                                                 n_tile * BLOCK_N + 64 * (box0 + b), first_row);
                 }
                 bulk_commit_group();
             };
             if (signaller) bulk_wait_group_read<0>();  // the previous stores have read the buffer
             wg_sync();
-            gemm_epilogue_tile<BLOCK_N, false, true, 0, JP>(p, acc, lane, row0, m_tile, n_tile, ph, s_stats, 0, stg);
+            gemm_epilogue_tile<BLOCK_N, false, true, 0, JP, PLAIN>(p, acc, lane, r0, m128, n_tile, ph, s_stats, 0, stg);
             fence_proxy_async();  // this thread's st.shared -> visible to the TMA store (async proxy)
             wg_sync();
-            if (signaller) store(0);
+            if (signaller) store(grow0, 0);
             if constexpr (PASSES == 2) {
                 if (signaller) bulk_wait_group_read<0>();
                 wg_sync();
                 gemm_epilogue_tile<BLOCK_N, false, true, JP, 2 * JP>(p, acc, lane, row0, m_tile, n_tile, ph, s_stats, 0, stg);
                 fence_proxy_async();
                 wg_sync();
-                if (signaller) store(JP / 8);
+                if (signaller) store(grow0, JP / 8);
+            }
+            if constexpr (MH == 2) {  // the second 64-row half, once the first half's stores have read the buffer
+                if (signaller) bulk_wait_group_read<0>();
+                wg_sync();
+                gemm_epilogue_tile<BLOCK_N, false, true, 0, JP, PLAIN>(p, acc + Cfg::ACC_REGS, lane, r0 + 64, m128, n_tile, ph, s_stats, 0,
+                                                                         stg);
+                fence_proxy_async();
+                wg_sync();
+                if (signaller) store(grow0 + 64, 0);
             }
         } else {
             gemm_epilogue_tile<BLOCK_N>(p, acc, lane, row0, m_tile, n_tile, ph, s_stats);
         }
     }
     if (OUT_TMA && signaller) bulk_wait_group<0>();  // the output is written before the CTA exits
-    if (p.stats != nullptr) {
+    if (!PLAIN && p.stats != nullptr) {
         asm volatile("bar.sync 1, 256;" ::: "memory");  // the two MMA warpgroups only
         const int n_tile = my_cta % p.num_n_tiles;      // fixed per CTA (num_ctas % num_n_tiles == 0)
         for (int i = threadIdx.x; i < BLOCK_N; i += 256) {
@@ -345,6 +381,12 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_fwd_tma_kernel(const __grid_
     gemm_fwd_body<BLOCK_N, NSPLIT, false, true>(p);
 }
 
+// 256-row tiles of the single-pass launches with a plain epilogue (pick_block_m).
+template <int BLOCK_N, int NSPLIT>
+__global__ void __launch_bounds__(kThreads, 1) gemm_fwd_tall_kernel(const __grid_constant__ GemmParams p) {
+    gemm_fwd_body<BLOCK_N, NSPLIT, false, true, 2 * kBlockM>(p);
+}
+
 // Per-group weights: the class-aware 1x1 output conv and its dgrad, where every crop (4096 rows) reads its class's weight rows.
 template <int BLOCK_N, int NSPLIT>
 __global__ void __launch_bounds__(kThreads, 1) gemm_fwd_grouped_kernel(const __grid_constant__ GemmParams p) {
@@ -354,10 +396,12 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_fwd_grouped_kernel(const __g
 // ------------------------------------------------------------------------------------------------
 // host side
 // ------------------------------------------------------------------------------------------------
-template <int BLOCK_N, int NSPLIT, bool GROUPED>
+template <int BLOCK_N, int NSPLIT, bool GROUPED, int BLOCK_M = kBlockM>
 static int launch_gemm(const GemmParams& p, cudaStream_t stream) {
-    using Cfg = GemmCfg<BLOCK_N, NSPLIT>;
-    auto kern = GROUPED ? gemm_fwd_grouped_kernel<BLOCK_N, NSPLIT>
+    using Cfg = GemmCfg<BLOCK_N, NSPLIT, BLOCK_M>;
+    void (*kern)(const GemmParams);
+    if constexpr (BLOCK_M != kBlockM) kern = gemm_fwd_tall_kernel<BLOCK_N, NSPLIT>;
+    else kern = GROUPED ? gemm_fwd_grouped_kernel<BLOCK_N, NSPLIT>
                         : (p.out_tma ? gemm_fwd_tma_kernel<BLOCK_N, NSPLIT> : gemm_fwd_kernel<BLOCK_N, NSPLIT>);
     static bool attr_set[2] = {false, false};
     if (!attr_set[p.out_tma]) {
@@ -389,11 +433,17 @@ static int launch_gemm(const GemmParams& p, cudaStream_t stream) {
     return 0;
 }
 
-static thread_local int g_last_variant = 0;
+static thread_local int g_last_variant = 0, g_last_block_m = 0;
 
+// p.num_m_tiles counts tiles of block_m rows
 template <bool GROUPED>
-static int dispatch_gemm(const GemmParams& p, int block_n, int nsplit, cudaStream_t stream) {
+static int dispatch_gemm(const GemmParams& p, int block_n, int block_m, int nsplit, cudaStream_t stream) {
     g_last_variant = block_n * 10 + nsplit;
+    g_last_block_m = block_m;
+    if (block_m != kBlockM) {
+        if (!GROUPED && block_m == 2 * kBlockM && block_n == 128 && nsplit == 1) return launch_gemm<128, 1, false, 2 * kBlockM>(p, stream);
+        return set_error(GDRN_ERR_ARG, "gemm: no %d-row tile for block_n=%d nsplit=%d", block_m, block_n, nsplit);
+    }
     if (nsplit == 1) {
         if (block_n == 128) return launch_gemm<128, 1, GROUPED>(p, stream);
         if (block_n == 64) return launch_gemm<64, 1, GROUPED>(p, stream);
@@ -404,8 +454,9 @@ static int dispatch_gemm(const GemmParams& p, int block_n, int nsplit, cudaStrea
     return set_error(GDRN_ERR_ARG, "gemm: unsupported block_n=%d nsplit=%d", block_n, nsplit);
 }
 
-static int dispatch_gemm(const GemmParams& p, int block_n, int nsplit, cudaStream_t stream) {
-    return p.group != nullptr ? dispatch_gemm<true>(p, block_n, nsplit, stream) : dispatch_gemm<false>(p, block_n, nsplit, stream);
+static int dispatch_gemm(const GemmParams& p, int block_n, int block_m, int nsplit, cudaStream_t stream) {
+    return p.group != nullptr ? dispatch_gemm<true>(p, block_n, block_m, nsplit, stream)
+                              : dispatch_gemm<false>(p, block_n, block_m, nsplit, stream);
 }
 
 // Grouped weights (gdrn_conv_fwd_grouped / gdrn_gemm_fwd_grouped): the argument checks shared by both, without touching the device.
@@ -444,6 +495,23 @@ static int pick_block_n(int n_pad, int num_m_tiles) {
     if (n_pad % 128 == 0 && num_m_tiles * (n_pad / 128) >= (num_sms() * 3) / 4) return 128;
     if (num_m_tiles * (n_pad / 128) < num_sms() / 2) return 64;
     return n_pad % 128 == 0 ? 128 : 64;
+}
+
+// Tile height, after pick_block_n has fixed the width from the 128-row tile count: 256 rows (gemm_fwd_tall_kernel) for a
+// single-pass 128-wide launch whose epilogue is plain -- a TMA-stored 16-bit plane (make_out_maps; so not grouped), no lo plane,
+// residual, fp32 output, BatchNorm statistics or output-parity phases -- while the 256-row tiles still fill >= ~0.75 waves.
+static int pick_block_m(const GemmParams& p, int block_n, int nsplit) {
+    const bool plain = p.out_tma && p.out_lo == nullptr && p.res_hi == nullptr && p.out_f32 == nullptr && p.stats == nullptr &&
+                       p.group == nullptr && p.nphase == 0;
+    const int tall_tiles = (p.M + 2 * kBlockM - 1) / (2 * kBlockM) * p.num_n_tiles;
+    return nsplit == 1 && block_n == 128 && plain && tall_tiles >= (num_sms() * 3) / 4 ? 2 * kBlockM : kBlockM;
+}
+
+// Sets the tile height and the M-tile count of a launch whose GemmParams are otherwise complete.
+static int set_block_m(GemmParams& p, int block_n, int nsplit) {
+    const int block_m = pick_block_m(p, block_n, nsplit);
+    p.num_m_tiles = (p.M + block_m - 1) / block_m;
+    return block_m;
 }
 
 }  // namespace gdrn
@@ -524,7 +592,7 @@ static int conv_fwd_impl(const void* x_hi, const void* x_lo, const void* w_hi, c
     p.num_w_groups = num_groups;
     p.bias_stride = bias_stride;
     if (make_out_maps(p, nsplit)) return GDRN_ERR_CUDA;
-    return dispatch_gemm(p, block_n, nsplit, stream);
+    return dispatch_gemm(p, block_n, set_block_m(p, block_n, nsplit), nsplit, stream);
 }
 
 extern "C" int gdrn_conv_fwd(const void* x_hi, const void* x_lo, const void* w_hi, const void* w_lo, void* y_hi,
@@ -634,7 +702,7 @@ extern "C" int gdrn_conv_dgrad_s2(const void* du_hi, const void* du_lo, const vo
     p.num_kb = nt * p.cchunks;  // bookkeeping only (per-tile counts come from the phase table)
     for (p.pw_log2 = 0; (1 << p.pw_log2) < Wo; ++p.pw_log2) {}
     for (p.ph_log2 = 0; (1 << p.ph_log2) < Ho; ++p.ph_log2) {}
-    return dispatch_gemm(p, block_n, nsplit, stream);
+    return dispatch_gemm(p, block_n, kBlockM, nsplit, stream);
 }
 
 static int gemm_fwd_impl(const void* a_hi, const void* a_lo, const void* w_hi, const void* w_lo, void* y_hi, void* y_lo,
@@ -682,7 +750,7 @@ static int gemm_fwd_impl(const void* a_hi, const void* a_lo, const void* w_hi, c
     p.num_w_groups = num_groups;
     p.bias_stride = bias_stride;
     if (make_out_maps(p, nsplit)) return GDRN_ERR_CUDA;
-    return dispatch_gemm(p, block_n, nsplit, stream);
+    return dispatch_gemm(p, block_n, set_block_m(p, block_n, nsplit), nsplit, stream);
 }
 
 extern "C" int gdrn_gemm_fwd(const void* a_hi, const void* a_lo, const void* w_hi, const void* w_lo, void* y_hi,
@@ -705,3 +773,6 @@ extern "C" int gdrn_gemm_fwd_grouped(const void* a_hi, const void* a_lo, const v
 
 // BLOCK_N * 10 + NSPLIT of the most recent gdrn_conv_fwd / gdrn_gemm_fwd call on this thread
 extern "C" int gdrn_last_gemm_variant() { return g_last_variant; }
+
+// tile height (128 or 256 rows) of the same call
+extern "C" int gdrn_last_gemm_block_m() { return g_last_block_m; }

@@ -32,6 +32,7 @@ int gdrn_storage_format(void); /* 0: bf16 (hi, lo) planes; 1: fp16 planes, lo = 
 float gdrn_lo_scale(void);
 int gdrn_set_pdl(int on); /* A/B: programmatic dependent launch of the GEMM kernels (prologue under the predecessor's tail); default on, GDRN_PDL=0 disables */
 int gdrn_last_gemm_variant(void); /* BLOCK_N*10 + nsplit of this thread's last conv/gemm forward launch */
+int gdrn_last_gemm_block_m(void); /* tile height (128 or 256 rows) of the same launch */
 
 /* ---- wgmma implicit-GEMM convolution, forward (and dgrad with flipped/transposed weights) ------------
  * replaces nn.Conv2d / nn.ConvTranspose2d forward: resnet_backbone.py:21-49,69-76 (torchvision BasicBlock),
