@@ -125,14 +125,31 @@ class RotWithRegionHead(_ParamsOnly):
 
 
 class ConvPnPNet(_ParamsOnly):
-    """reference models/conv_pnp_net.py:41-109 (drop_prob = 0, mask_attention 'none')."""
+    """reference models/conv_pnp_net.py:41-109 (mask_attention 'none').
+
+    DropBlock (PNP_HEAD_CFG.drop_prob > 0, conv_pnp_net.py:66-72,128-142): every forward, in train and in eval mode, advances
+    the LinearScheduler counter (np.linspace(0, drop_prob, 5000)[min(k, 4999)] at forward k); in train mode the Patch-PnP input
+    is multiplied by a block mask and numel / sum(mask).  The counter lives on the device (`dropblock_step` reads and sets it),
+    is not part of the state_dict and starts at 0 with every new module, like the reference's plain attribute.
+    `dropblock_seed` (default: derived from torch.initial_seed() at construction) keys the Philox generator of the mask
+    together with the data-parallel rank.  After a train forward, `dropblock_seeds`, `dropblock_keep` ([B, 64, 64] uint8) and
+    `dropblock_scale` ([1] fp32) are the device tensors of the mask it used."""
 
     def __init__(self, nIn, featdim=128, rot_dim=6, num_layers=3, norm="GN", num_gn_groups=32, num_regions=64,
                  drop_prob=0.0, dropblock_size=5, mask_attention_type="none"):
         super().__init__()
-        if norm != "GN" or num_layers != 3 or featdim != 128 or drop_prob != 0.0 or mask_attention_type != "none":
-            raise NotImplementedError("only the a6 Patch-PnP (3 stride-2 convs, GN, featdim 128, no dropblock) is implemented")
+        if norm != "GN" or num_layers != 3 or featdim != 128 or mask_attention_type != "none":
+            raise NotImplementedError("only the a6 Patch-PnP (3 stride-2 convs, GN, featdim 128) is implemented")
+        if not 0.0 <= float(drop_prob) <= 1.0:
+            raise NotImplementedError(f"PNP_HEAD_CFG.drop_prob = {drop_prob!r} (0 <= drop_prob <= 1)")
+        if int(dropblock_size) != dropblock_size or not 1 <= dropblock_size <= 15:
+            raise NotImplementedError(f"PNP_HEAD_CFG.dropblock_size = {dropblock_size!r} (1..15)")
         self.featdim, self.num_regions, self.nIn, self.rot_dim = featdim, num_regions, nIn, rot_dim
+        self.drop_prob, self.dropblock_size = float(drop_prob), int(dropblock_size)
+        self.dropblock_seed = torch.initial_seed()
+        self._db_step = None  # int64 [1] on the device, created by dropblock_counter
+        self._db_bufs = {}    # batch size -> (keep, seeds, counts, scale), patch_pnp.dropblock_step
+        self.dropblock_seeds = self.dropblock_keep = self.dropblock_scale = None
         f = nn.ModuleList()
         for i in range(3):
             f.append(nn.Conv2d(nIn if i == 0 else featdim, featdim, 3, 2, 1, bias=False))
@@ -154,6 +171,23 @@ class ConvPnPNet(_ParamsOnly):
         self.precision = "fp32x3"  # stand-alone forward: "fp32x3" (1e-3 parity) | "half"
         self._runner = None
 
+    def dropblock_counter(self, device) -> torch.Tensor:
+        """The device-resident DropBlock step counter (int64 [1]) on `device`."""
+        if self._db_step is None:
+            self._db_step = torch.zeros(1, dtype=torch.int64, device=device)
+        elif self._db_step.device != torch.device(device):
+            self._db_step = self._db_step.to(device)
+        return self._db_step
+
+    @property
+    def dropblock_step(self) -> int:
+        """Forwards counted by the DropBlock schedule so far (the reference's `dropblock.i`); settable, e.g. to resume."""
+        return 0 if self._db_step is None else int(self._db_step.item())
+
+    @dropblock_step.setter
+    def dropblock_step(self, k: int):
+        self.dropblock_counter(self.fc1.weight.device).fill_(int(k))
+
     def forward(self, coor_feat, region=None, extents=None, mask_attention=None):
         """Stand-alone Patch-PnP inference with the reference signature (conv_pnp_net.py:111): xyz(+2-D coords) maps
         [B, 3|5, 64, 64], region attention [B, R, 64, 64] or None, extents [B, 3] -> (rot [B, rot_dim], t [B, 3]).
@@ -165,7 +199,7 @@ class ConvPnPNet(_ParamsOnly):
 
         if self._runner is None or self._runner.precision != {"mixed": "fp32x3"}.get(self.precision, self.precision):
             self._runner = PatchPnP(self, self.precision)
-        return self._runner(coor_feat, region, extents)
+        return self._runner(coor_feat, region, extents, train=self.training)
 
 
 def get_xyz_mask_region_out_dim(cfg):

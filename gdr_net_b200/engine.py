@@ -22,7 +22,7 @@ import torch
 from . import ops
 from .capi import C
 from .ops import PT, _stream
-from .patch_pnp import pnp_net_forward
+from .patch_pnp import dropblock_step, pnp_net_forward
 
 LOSS_NAMES = ["loss_coor_x", "loss_coor_y", "loss_coor_z", "loss_mask", "loss_region", "loss_PM_R", "loss_centroid", "loss_z"]
 MASK_LOSSES = {"L1": 0, "BCE": 1, "CE": 2}  # ROT_HEAD.MASK_LOSS_TYPE -> the mask_loss argument of the gdrn_*_ex loss kernels
@@ -223,6 +223,11 @@ class Engine:
         self.pnp_ld = -(-n_in // 64) * 64
         # the shipped head (64 regions with attention) runs the gdrn_*_ex loss kernels, every other one the gdrn_*_ex2 ones
         self.regions_ex2 = not (self.num_regions == 64 and self.region_att)
+        # DropBlock on the Patch-PnP input (PNP_HEAD_CFG.drop_prob, dropblock_size; ConvPnPNet): with drop_prob > 0 every forward
+        # advances the device-resident schedule counter and a train-mode one runs the gdrn_*_db glue and head backward
+        self.drop_prob = float(model.pnp_net.drop_prob)
+        if self.drop_prob > 0:
+            model.pnp_net.dropblock_counter(self.dev)
         # mask head (GDRN.py:339-400): MASK_LOSS_TYPE, the mask logits per pixel (1, or 2 for CE) and the GT mask of the xyz, mask
         # and region losses (XYZ_LOSS_MASK_GT, MASK_LOSS_GT, REGION_LOSS_MASK_GT)
         self.mask_loss = MASK_LOSSES[rh.MASK_LOSS_TYPE]
@@ -501,7 +506,7 @@ class Engine:
             if up:
                 cur = ops.upsample2x_fwd(cur)
             cur = cbr(cur, f"rot_head_net.features.{ci}", f"rot_head_net.features.{bi}", hf[ci])
-        return self._tail_inference(cur, aux, want_maps)
+        return self._tail_inference(cur, aux, want_maps, train=False)
 
     def _eval_graphed(self, x: torch.Tensor, aux: dict, want_maps: bool) -> dict:
         """Inference forward replayed as ONE CUDA graph per input signature (`use_cuda_graphs`): ~230 launches incl. the
@@ -521,10 +526,11 @@ class Engine:
         graph.replay()
         return {k: (v.clone() if isinstance(v, torch.Tensor) else v) for k, v in res.items()}
 
-    def _head_pnp(self, head_in: PT, aux: dict, pnp_saved: Optional[list] = None):
+    def _head_pnp(self, head_in: PT, aux: dict, pnp_saved: Optional[list] = None, train: bool = False):
         """1x1 output conv -> glue -> Patch-PnP (GDRN.py:156-181, conv_pnp_net.py:111-157).  Returns the fp32 logits
-        [B*4096, 72] (n_logits valid), the Patch-PnP input planes [B, 64, 64, pnp_ld], pred [B, 16] (cols 0..5 rot6d, 6..8 centroid dx, dy and z) and the inputs
-        of the three FC layers; pnp_saved receives the Patch-PnP conv activations (pnp_net_forward)."""
+        [B*4096, 72] (n_logits valid), the Patch-PnP input planes [B, 64, 64, pnp_ld], pred [B, 16] (cols 0..5 rot6d, 6..8 centroid dx, dy and z), the inputs
+        of the three FC layers and the DropBlock (keep, scale) of a train-mode forward with drop_prob > 0, else None; pnp_saved
+        receives the Patch-PnP conv activations (pnp_net_forward)."""
         m, B, dev = self.model, head_in.shape[0], self.dev
         logits = torch.empty(B * 4096, 72, device=dev)
         if self.class_aware:  # crop b (4096 rows) reads the weight / bias block of class roi_classes[b]
@@ -536,18 +542,22 @@ class Engine:
         pnp_in = PT((B, 64, 64, self.pnp_ld), self.planes, device=dev)
         glue = (logits.data_ptr(), ops.ptr(aux.get("roi_coord_2d")), aux["roi_extents"].data_ptr(), pnp_in.hi_ptr, pnp_in.lo_ptr, B, 4096,
                 self.with_2d, self.mask_out)
-        if self.regions_ex2:
+        db = dropblock_step(m.pnp_net, B, train, dev) if self.drop_prob > 0 else None
+        if db is not None:
+            C.gdrn_head_glue_fwd_db(*glue, self.num_regions, self.region_att, self.pnp_ld, db[0].data_ptr(), db[1].data_ptr(), _stream())
+        elif self.regions_ex2:
             C.gdrn_head_glue_fwd_ex2(*glue, self.num_regions, self.region_att, self.pnp_ld, _stream())
         else:
             C.gdrn_head_glue_fwd_ex(*glue, _stream())
         pred = torch.zeros(B, 16, device=dev)
         fc_in = pnp_net_forward(pnp_in, m.pnp_net, self.wf, self.b_rt, pred, pnp_saved)
-        return logits, pnp_in, pred, fc_in
+        return logits, pnp_in, pred, fc_in, db
 
-    def _tail_inference(self, head_in: PT, aux: dict, want_maps: bool) -> dict:
-        """1x1 output conv -> glue -> Patch-PnP -> test-time pose decode (shared by the folded and the plain eval forward)."""
+    def _tail_inference(self, head_in: PT, aux: dict, want_maps: bool, train: bool) -> dict:
+        """1x1 output conv -> glue -> Patch-PnP -> test-time pose decode (shared by the folded and the plain eval forward);
+        train: DropBlock applies (a train-mode forward without losses)."""
         B = head_in.shape[0]
-        logits, _, pred, _ = self._head_pnp(head_in, aux)
+        logits, _, pred, _, _ = self._head_pnp(head_in, aux, train=train)
         out_rot = torch.empty(B, 3, 3, device=self.dev)
         out_trans = torch.empty(B, 3, device=self.dev)
         C.gdrn_pose_loss(pred.data_ptr(), 16, aux["roi_cams"].data_ptr(), aux["roi_centers"].data_ptr(),
@@ -767,11 +777,11 @@ class Engine:
         if self._nbt:
             torch._foreach_add_(self._nbt, 1)  # all BatchNorm num_batches_tracked counters in one launch
         if not do_loss:
-            return self._tail_inference(head_in, aux, want_maps)
+            return self._tail_inference(head_in, aux, want_maps, train=train_bn)
 
         # ---- a3 + a4: glue and Patch-PnP
         pnp_saved = []
-        logits, pnp_in, pred, (flat, h1, h2) = self._head_pnp(head_in, aux, pnp_saved)
+        logits, pnp_in, pred, (flat, h1, h2), db = self._head_pnp(head_in, aux, pnp_saved, train=train_bn)
 
         # ---- a5/a6 pose decode + a7..a10 losses
         if self.live_head:
@@ -786,7 +796,7 @@ class Engine:
         else:  # frozen head: no per-pixel losses; the finalize kernel's first five outputs are dropped below
             pix_sums = torch.zeros(7, dtype=torch.float64, device=dev)
         S.update(logits=logits, pnp_in=pnp_in, pnp=pnp_saved, flat=flat, h1=h1, h2=h2, pred=pred, head_in=head_in if keep_head else None,
-                 pix_sums=pix_sums, aux=aux)
+                 pix_sums=pix_sums, aux=aux, db=db)
         self.saved = S
         # the pose kernel needs the upstream loss gradients to emit dY9; forward calls it with unit weights and
         # backward re-runs it (cheap: B CTAs) with the actual ones.
@@ -965,7 +975,10 @@ class Engine:
         hb = (S["logits"].data_ptr(), aux["gt_xyz"].data_ptr(), m_xyz, m_mask, m_region, aux["gt_region"].data_ptr(),
               S["pix_sums"].data_ptr(), gw.data_ptr(), d_pnp_in.hi_ptr, d_pnp_in.lo_ptr, aux["roi_extents"].data_ptr(), dlog.hi_ptr,
               dlog.lo_ptr, B, 4096, self.with_2d, self.mask_loss, self.mask_out)
-        if self.regions_ex2:
+        if S["db"] is not None:
+            C.gdrn_head_bwd_db(*hb, self.num_regions, self.region_att, self.pnp_ld, S["db"][0].data_ptr(), S["db"][1].data_ptr(),
+                               _stream())
+        elif self.regions_ex2:
             C.gdrn_head_bwd_ex2(*hb, self.num_regions, self.region_att, self.pnp_ld, _stream())
         else:
             C.gdrn_head_bwd_ex(*hb, _stream())
@@ -1116,8 +1129,10 @@ def _capture(engine: "Engine", steps, warmup: int, restore_bn: bool = False, poo
     """Runs `warmup` rounds of the callables `steps` on a side stream (this also sizes the split-K workspace and uploads the
     pack job tables), then captures each step into its own CUDA graph, all in `pool` if one is given.  Returns
     [(graph, what the step returned)].  restore_bn: the warm-up leaves the BatchNorm running statistics and counters as
-    they were."""
+    they were.  The DropBlock step counter is always restored: a replayed run sees the same mask sequence as an eager one."""
     bn_bufs = [t for m in engine._bn_mods.values() for t in m.buffers()] if restore_bn else []
+    if engine.drop_prob > 0:
+        bn_bufs.append(engine.model.pnp_net.dropblock_counter(engine.dev))
     snap = [t.clone() for t in bn_bufs]
     side = torch.cuda.Stream()
     side.wait_stream(torch.cuda.current_stream())

@@ -217,6 +217,31 @@ int gdrn_head_bwd_ex2(const float* logits, const float* gt_xyz, const float* m_x
 int gdrn_pnp_pack_input_ex(const float* coor_feat, int c_feat, const float* region, int c_reg, const float* extents,
                            void* out_hi, void* out_lo, int B, int HW, int pnp_ld, void* stream);
 
+/* ---- DropBlock on the Patch-PnP input (PNP_NET.PNP_HEAD_CFG.drop_prob / dropblock_size; conv_pnp_net.py:66-72,128-142,
+ * core/utils/dropblock).  *step (device int64) is the LinearScheduler counter k: the step's probability is
+ * np.linspace(0, drop_prob, 5000)[min(k, 4999)], computed on the device in float64, and every call adds 1 to *step.
+ * train = 1 also samples the block mask of B crops of H x W pixels (H, W <= 64): seeds[B][H][W] = (uniform < float32(p /
+ * block_size^2)) from Philox4x32-10 with key (seed, rank) and counter (pixel quad, crop, k); keep[B][H][W] = 1 - max_pool2d(seeds,
+ * block_size, stride 1, padding block_size / 2) (even sizes crop the last row and column); counts[B] the per-crop kept
+ * pixels; scale[0] = B H W / sum(counts).  train = 0 only advances *step (keep, seeds, counts, scale may be NULL).
+ * drop_prob outside [0, 1], block_size outside 1..15 or H, W outside 1..64 give GDRN_ERR_ARG. */
+int gdrn_dropblock_step(long long* step, long long seed, int rank, double drop_prob, int block_size, int train,
+                        unsigned char* keep, unsigned char* seeds, int* counts, float* scale, int B, int H, int W, void* stream);
+/* gdrn_head_glue_fwd_ex2, gdrn_head_bwd_ex2 and gdrn_pnp_pack_input_ex with DropBlock: each valid Patch-PnP input channel of
+ * pixel p is multiplied by keep[p] * scale[0] in fp32 before the 16-bit split (forward), and each d(Patch-PnP input) row by
+ * the same factor before its use (backward).  head_bwd_db runs its own kernels for every region setting, 64 regions with
+ * attention included. */
+int gdrn_head_glue_fwd_db(const float* logits, const float* coord2d, const float* extents, void* out_hi, void* out_lo, int B,
+                          int HW, int with_2d, int mask_out, int num_regions, int region_att, int pnp_ld,
+                          const unsigned char* keep, const float* scale, void* stream);
+int gdrn_head_bwd_db(const float* logits, const float* gt_xyz, const float* m_xyz, const float* m_mask, const float* m_region,
+                     const long long* labels, const double* sums, const float* gw, const void* din_hi, const void* din_lo,
+                     const float* extents, void* out_hi, void* out_lo, int B, int HW, int with_2d, int mask_loss, int mask_out,
+                     int num_regions, int region_att, int pnp_ld, const unsigned char* keep, const float* scale, void* stream);
+int gdrn_pnp_pack_input_db(const float* coor_feat, int c_feat, const float* region, int c_reg, const float* extents,
+                           void* out_hi, void* out_lo, int B, int HW, int pnp_ld, const unsigned char* keep, const float* scale,
+                           void* stream);
+
 /* ---- rot6d -> R, SITE translation, allo -> ego, PM loss (+ closest symmetric GT), centroid / z losses, re/te
  * (rot_reps.py:34-49, pose_from_pred_centroid_z.py:144-227, utils.py:208-236, pm_loss.py:82-114,
  *  pose_utils.py:430-482, GDRN.py:439-471, model_utils.py:40-52).  pred [B][ld_pred]: cols 0..5 rot6d, 6..8 t.
