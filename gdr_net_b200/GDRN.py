@@ -91,25 +91,30 @@ class ResNetBackboneNet(_ParamsOnly):
 class RotWithRegionHead(_ParamsOnly):
     """reference models/cdpn_rot_head_region.py:10-143 (ROT_CONCAT=False branch; concat mode is broken
     upstream, SURVEY P8).  `features` keeps the reference indices: ReLU / upsample placeholders included.
-    With rot / mask / region_class_aware the output conv carries that block once per class (engine.class_rows)."""
+    With rot / mask / region_class_aware the output conv carries that block once per class (engine.class_rows).
+    norm = "BN" (nn.BatchNorm2d) or "GN" (nn.GroupNorm(num_gn_groups, 256), layer_utils.get_norm) at 1, 4, 7, 11, 14, 18, 21."""
 
     def __init__(self, in_channels=512, num_layers=3, num_filters=256, kernel_size=3, output_kernel_size=1,
-                 rot_output_dim=3, mask_output_dim=1, num_regions=64, norm="BN", freeze=False, num_classes=1,
+                 rot_output_dim=3, mask_output_dim=1, num_regions=64, norm="BN", num_gn_groups=32, freeze=False, num_classes=1,
                  rot_class_aware=False, mask_class_aware=False, region_class_aware=False):
         super().__init__()
-        if kernel_size != 3 or output_kernel_size != 1 or norm != "BN" or num_layers != 3:
+        check_head_norm(norm, num_gn_groups)
+        if kernel_size != 3 or output_kernel_size != 1 or num_layers != 3:
             raise NotImplementedError("only the a6 head (k3 deconv, 1x1 output conv, BN, 3 stages) is implemented")
         self.freeze = freeze
         f = nn.ModuleList()
+        def norm_layer():
+            return nn.GroupNorm(num_gn_groups, num_filters) if norm == "GN" else nn.BatchNorm2d(num_filters)
+
         f.append(nn.ConvTranspose2d(in_channels, num_filters, 3, stride=2, padding=1, output_padding=1, bias=False))
-        f.append(nn.BatchNorm2d(num_filters))
+        f.append(norm_layer())
         f.append(nn.ReLU(inplace=True))
         for i in range(num_layers):
             if i >= 1:
                 f.append(nn.UpsamplingBilinear2d(scale_factor=2))
             for _ in range(2):
                 f.append(nn.Conv2d(num_filters, num_filters, 3, 1, 1, bias=False))
-                f.append(nn.BatchNorm2d(num_filters))
+                f.append(norm_layer())
                 f.append(nn.ReLU(inplace=True))
         self.rot_output_dim = rot_output_dim * (num_classes if rot_class_aware else 1)
         self.mask_output_dim = mask_output_dim * (num_classes if mask_class_aware else 1)
@@ -119,9 +124,18 @@ class RotWithRegionHead(_ParamsOnly):
         for m in self.modules():
             if isinstance(m, (nn.Conv2d, nn.ConvTranspose2d)):
                 _normal_init(m, 0.001)
-            elif isinstance(m, nn.BatchNorm2d):
+            elif isinstance(m, (nn.BatchNorm2d, nn.GroupNorm)):
                 nn.init.constant_(m.weight, 1.0)
                 nn.init.constant_(m.bias, 0.0)
+
+
+def check_head_norm(norm, num_gn_groups):
+    """ROT_HEAD.NORM / NUM_GN_GROUPS: BatchNorm, or GroupNorm with a group count that divides 256 and is at most 64 (the
+    gdrn_head_gn_* kernels); anything else raises NotImplementedError naming the key."""
+    if norm not in ("BN", "GN"):
+        raise NotImplementedError(f"ROT_HEAD.NORM = {norm!r} (BN or GN)")
+    if norm == "GN" and (int(num_gn_groups) != num_gn_groups or not 1 <= num_gn_groups <= 64 or 256 % int(num_gn_groups)):
+        raise NotImplementedError(f"ROT_HEAD.NUM_GN_GROUPS = {num_gn_groups!r} (a divisor of 256, at most 64)")
 
 
 class ConvPnPNet(_ParamsOnly):
@@ -231,6 +245,10 @@ def _check_supported(cfg):
         problems.append("backbone must be resnet18/34 at 256 -> 64")
     if r.ROT_CONCAT:
         problems.append("concat heads (ROT_HEAD.ROT_CONCAT)")
+    try:
+        check_head_norm(r.NORM, r.get("NUM_GN_GROUPS", 32))
+    except NotImplementedError as e:
+        problems.append(str(e))
     if (r.ROT_CLASS_AWARE or r.MASK_CLASS_AWARE or r.REGION_CLASS_AWARE) and not int(r.NUM_CLASSES) >= 1:
         problems.append(f"ROT_HEAD.NUM_CLASSES = {r.NUM_CLASSES!r} with a class-aware head (>= 1)")
     if r.XYZ_LOSS_TYPE != "L1" or r.MASK_LOSS_TYPE not in ("L1", "BCE", "CE") or r.REGION_LOSS_TYPE != "CE":
@@ -420,7 +438,7 @@ def build_model_optimizer(cfg, precision: str = "mixed"):
     rot_head_net = RotWithRegionHead(
         channels[-1], r_head_cfg.NUM_LAYERS, r_head_cfg.NUM_FILTERS, r_head_cfg.CONV_KERNEL_SIZE,
         r_head_cfg.OUT_CONV_KERNEL_SIZE, rot_output_dim=r_out_dim, mask_output_dim=mask_out_dim,
-        num_regions=r_head_cfg.NUM_REGIONS, norm=r_head_cfg.NORM, freeze=r_head_cfg.FREEZE,
+        num_regions=r_head_cfg.NUM_REGIONS, norm=r_head_cfg.NORM, num_gn_groups=r_head_cfg.NUM_GN_GROUPS, freeze=r_head_cfg.FREEZE,
         num_classes=r_head_cfg.NUM_CLASSES, rot_class_aware=r_head_cfg.ROT_CLASS_AWARE,
         mask_class_aware=r_head_cfg.MASK_CLASS_AWARE, region_class_aware=r_head_cfg.REGION_CLASS_AWARE,
     )

@@ -1084,6 +1084,232 @@ __global__ void leaky_bwd_kernel(const bf16* __restrict__ g_hi, const bf16* __re
     }
 }
 
+// ------------------------------------------------------------------------------------------------
+// GroupNorm(G, 256) + ReLU of the geometry head (ROT_HEAD.NORM = "GN"; cdpn_rot_head_region.py with get_norm("GN")), tensor
+// [B][HW][256], HW in {256, 1024, 4096}.  Every reduction has a fixed decomposition and a fixed order, no atomics: the same
+// inputs give bit-identical statistics and gradients on every run.  A crop is split into S = gn_head_splits(HW) slices of
+// HW / S rows, one CTA per (slice, crop), so B = 4 already launches 128 CTAs at 64 x 64.
+//   forward   stats_partial (per slice and group: sum x, sum x^2; fp32 per thread over <= 16 rows, double beyond) ->
+//             stats_final (per crop and group, slices in order: mean, invstd) -> apply (relu(gamma x^ + beta) in fp32 before the
+//             16-bit split, and the ReLU bitmap of the BatchNorm path: bit j of byte i = element 8 i + j > 0)
+//   backward  bwd_partial (per slice and channel: sum dy, sum dy x^, dy masked by the bitmap) -> bwd_crop (per crop, slices in
+//             order: the channel sums and the group means of gamma dy, gamma dy x^) -> bwd_param (dbeta, dgamma: crops in
+//             order) -> bwd_apply (dx = invstd (gamma dy - mean(gamma dy) - x^ mean(gamma dy x^)))
+// ------------------------------------------------------------------------------------------------
+constexpr int kGnHeadC = 256;
+constexpr int kGnHeadLanes = 8;  // row lanes per CTA: 256 threads = 32 column groups of 8 channels x 8 lanes
+
+__host__ __device__ __forceinline__ int gn_head_splits(int HW) { return HW / 32 < 32 ? HW / 32 : 32; }
+
+// workspace (doubles): forward partials [B][S][G][2]; backward partials [B][S][2][256] floats, then the crop sums
+// [B][2][256] doubles, then the group means [B][G][2] floats
+__host__ __device__ __forceinline__ long gn_head_ws_crop(int B, int S) { return (long)B * S * kGnHeadC; }
+__host__ __device__ __forceinline__ long gn_head_ws_gred(int B, int S) { return gn_head_ws_crop(B, S) + (long)B * 2 * kGnHeadC; }
+
+__global__ void __launch_bounds__(256) gn_head_stats_partial_kernel(const bf16* __restrict__ u_hi, const bf16* __restrict__ u_lo,
+                                                                    double* __restrict__ part, int HW, int G) {
+    const int s = blockIdx.x, S = gridDim.x, b = blockIdx.y;
+    const int col = threadIdx.x % 32, rl = threadIdx.x / 32;
+    const int R = HW / S, cpg = kGnHeadC / G;
+    __shared__ float red[2][kGnHeadLanes][kGnHeadC + 4];
+    __shared__ double chs[2][kGnHeadC];
+    float s0[8], s1[8];
+#pragma unroll
+    for (int j = 0; j < 8; ++j) s0[j] = s1[j] = 0.f;
+    const long base = ((long)b * HW + (long)s * R) * 32 + col;
+#pragma unroll 4
+    for (int r = rl; r < R; r += kGnHeadLanes) {
+        float v[8];
+        load8(u_hi, u_lo, base + (long)r * 32, v);
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+            s0[j] += v[j];
+            s1[j] = fmaf(v[j], v[j], s1[j]);
+        }
+    }
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+        red[0][rl][col * 8 + j] = s0[j];
+        red[1][rl][col * 8 + j] = s1[j];
+    }
+    __syncthreads();
+    {
+        const int c = threadIdx.x;
+        double a0 = 0.0, a1 = 0.0;
+        for (int q = 0; q < kGnHeadLanes; ++q) {
+            a0 += (double)red[0][q][c];
+            a1 += (double)red[1][q][c];
+        }
+        chs[0][c] = a0;
+        chs[1][c] = a1;
+    }
+    __syncthreads();
+    if (threadIdx.x < 2 * G) {
+        const int grp = threadIdx.x >> 1, k = threadIdx.x & 1;
+        double a = 0.0;
+        for (int c = grp * cpg; c < (grp + 1) * cpg; ++c) a += chs[k][c];
+        part[(((long)b * S + s) * G + grp) * 2 + k] = a;
+    }
+}
+
+__global__ void gn_head_stats_final_kernel(const double* __restrict__ part, float* __restrict__ stats, int B, int S, int G,
+                                           double n, float eps) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;  // (crop, group)
+    if (i >= B * G) return;
+    const int b = i / G, grp = i % G;
+    double a0 = 0.0, a1 = 0.0;
+    for (int s = 0; s < S; ++s) {
+        a0 += part[(((long)b * S + s) * G + grp) * 2 + 0];
+        a1 += part[(((long)b * S + s) * G + grp) * 2 + 1];
+    }
+    const double m = a0 / n;
+    double var = a1 / n - m * m;
+    if (var < 0.0) var = 0.0;
+    stats[(long)i * 2 + 0] = (float)m;
+    stats[(long)i * 2 + 1] = (float)(1.0 / sqrt(var + (double)eps));
+}
+
+// the per-channel (mean, invstd) of 8 consecutive channels c0.. of crop b: at most two groups (C / G >= 4)
+__device__ __forceinline__ void gn_head_channel_stats(const float* __restrict__ stats, int b, int c0, int G, float (&mu)[8],
+                                                      float (&rs)[8]) {
+    const int cpg = kGnHeadC / G;
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+        const long k = ((long)b * G + (c0 + j) / cpg) * 2;
+        mu[j] = __ldg(stats + k);
+        rs[j] = __ldg(stats + k + 1);
+    }
+}
+
+__global__ void __launch_bounds__(256) gn_head_apply_kernel(const bf16* __restrict__ u_hi, const bf16* __restrict__ u_lo,
+                                                            bf16* __restrict__ y_hi, bf16* __restrict__ y_lo,
+                                                            uint8_t* __restrict__ mask_out, const float* __restrict__ gamma,
+                                                            const float* __restrict__ beta, const float* __restrict__ stats,
+                                                            long n8, int HW, int G) {
+    for (long idx = blockIdx.x * (long)blockDim.x + threadIdx.x; idx < n8; idx += (long)gridDim.x * blockDim.x) {
+        const int c0 = (int)(idx % 32) * 8;
+        const int b = (int)(idx / 32 / HW);
+        float v[8], mu[8], rs[8];
+        load8(u_hi, u_lo, idx, v);
+        gn_head_channel_stats(stats, b, c0, G, mu, rs);
+        uint32_t bits = 0;
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+            const float sc = __ldg(gamma + c0 + j) * rs[j];
+            v[j] = fmaxf(fmaf(v[j], sc, fmaf(-mu[j], sc, __ldg(beta + c0 + j))), 0.f);
+            bits |= (v[j] > 0.f ? 1u : 0u) << j;
+        }
+        store8(y_hi, y_lo, idx, v);
+        if (mask_out != nullptr) mask_out[idx] = (uint8_t)bits;
+    }
+}
+
+__global__ void __launch_bounds__(256) gn_head_bwd_partial_kernel(const bf16* __restrict__ g_hi, const bf16* __restrict__ g_lo,
+                                                                  const bf16* __restrict__ u_hi, const bf16* __restrict__ u_lo,
+                                                                  const uint8_t* __restrict__ mask_in,
+                                                                  const float* __restrict__ stats, float* __restrict__ part,
+                                                                  int HW, int G) {
+    const int s = blockIdx.x, S = gridDim.x, b = blockIdx.y;
+    const int col = threadIdx.x % 32, rl = threadIdx.x / 32;
+    const int R = HW / S;
+    __shared__ float red[2][kGnHeadLanes][kGnHeadC + 4];
+    float mu[8], rs[8], s0[8], s1[8];
+    gn_head_channel_stats(stats, b, col * 8, G, mu, rs);
+#pragma unroll
+    for (int j = 0; j < 8; ++j) s0[j] = s1[j] = 0.f;
+    const long base = ((long)b * HW + (long)s * R) * 32 + col;
+#pragma unroll 4
+    for (int r = rl; r < R; r += kGnHeadLanes) {
+        const long off = base + (long)r * 32;
+        float gv[8], u[8];
+        load8(g_hi, g_lo, off, gv);
+        load8(u_hi, u_lo, off, u);
+        const uint32_t bits = __ldg(mask_in + off);
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+            const float gg = ((bits >> j) & 1u) ? gv[j] : 0.f;
+            s0[j] += gg;
+            s1[j] = fmaf(gg, (u[j] - mu[j]) * rs[j], s1[j]);
+        }
+    }
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+        red[0][rl][col * 8 + j] = s0[j];
+        red[1][rl][col * 8 + j] = s1[j];
+    }
+    __syncthreads();
+    const int c = threadIdx.x;
+    float a0 = 0.f, a1 = 0.f;
+    for (int q = 0; q < kGnHeadLanes; ++q) {
+        a0 += red[0][q][c];
+        a1 += red[1][q][c];
+    }
+    float* out = part + (((long)b * S + s) * 2) * kGnHeadC;
+    out[c] = a0;
+    out[kGnHeadC + c] = a1;
+}
+
+// one CTA per crop: channel sums over the slices (kept for the parameter gradients) and the group means of gamma dy, gamma dy x^
+__global__ void __launch_bounds__(256) gn_head_bwd_crop_kernel(const float* __restrict__ part, const float* __restrict__ gamma,
+                                                               double* __restrict__ crop, float* __restrict__ gred, int S, int G,
+                                                               double n) {
+    const int b = blockIdx.x, c = threadIdx.x, cpg = kGnHeadC / G;
+    __shared__ double gs[2][kGnHeadC];
+    double a0 = 0.0, a1 = 0.0;
+    const float* p = part + (long)b * S * 2 * kGnHeadC + c;
+    for (int s = 0; s < S; ++s) {
+        a0 += (double)__ldg(p + (2L * s) * kGnHeadC);
+        a1 += (double)__ldg(p + (2L * s + 1) * kGnHeadC);
+    }
+    crop[((long)b * 2) * kGnHeadC + c] = a0;
+    crop[((long)b * 2 + 1) * kGnHeadC + c] = a1;
+    const double ga = (double)__ldg(gamma + c);
+    gs[0][c] = a0 * ga;
+    gs[1][c] = a1 * ga;
+    __syncthreads();
+    if (threadIdx.x < 2 * G) {
+        const int grp = threadIdx.x >> 1, k = threadIdx.x & 1;
+        double a = 0.0;
+        for (int q = grp * cpg; q < (grp + 1) * cpg; ++q) a += gs[k][q];
+        gred[((long)b * G + grp) * 2 + k] = (float)(a / n);
+    }
+}
+
+// dbeta[c] = sum over crops of sum dy, dgamma[c] = sum over crops of sum dy x^ (crops in order)
+__global__ void __launch_bounds__(256) gn_head_bwd_param_kernel(const double* __restrict__ crop, float* __restrict__ dgamma,
+                                                                float* __restrict__ dbeta, int B) {
+    const int c = threadIdx.x, k = blockIdx.x;  // k = 0: dbeta, 1: dgamma
+    double a = 0.0;
+    for (int b = 0; b < B; ++b) a += crop[((long)b * 2 + k) * kGnHeadC + c];
+    (k == 0 ? dbeta : dgamma)[c] = (float)a;
+}
+
+__global__ void __launch_bounds__(256) gn_head_bwd_apply_kernel(const bf16* __restrict__ g_hi, const bf16* __restrict__ g_lo,
+                                                                const bf16* __restrict__ u_hi, const bf16* __restrict__ u_lo,
+                                                                const uint8_t* __restrict__ mask_in, const float* __restrict__ gamma,
+                                                                const float* __restrict__ stats, const float* __restrict__ gred,
+                                                                bf16* __restrict__ du_hi, bf16* __restrict__ du_lo, long n8, int HW,
+                                                                int G) {
+    const int cpg = kGnHeadC / G;
+    for (long idx = blockIdx.x * (long)blockDim.x + threadIdx.x; idx < n8; idx += (long)gridDim.x * blockDim.x) {
+        const int c0 = (int)(idx % 32) * 8;
+        const int b = (int)(idx / 32 / HW);
+        float gv[8], u[8], mu[8], rs[8], o[8];
+        load8(g_hi, g_lo, idx, gv);
+        load8(u_hi, u_lo, idx, u);
+        const uint32_t bits = __ldg(mask_in + idx);
+        gn_head_channel_stats(stats, b, c0, G, mu, rs);
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+            const long k = ((long)b * G + (c0 + j) / cpg) * 2;
+            const float gg = ((bits >> j) & 1u) ? gv[j] : 0.f;
+            const float xh = (u[j] - mu[j]) * rs[j];
+            o[j] = rs[j] * (fmaf(gg, __ldg(gamma + c0 + j), -__ldg(gred + k)) - xh * __ldg(gred + k + 1));
+        }
+        store8(du_hi, du_lo, idx, o);
+    }
+}
+
 }  // namespace gdrn
 
 using namespace gdrn;
@@ -1344,5 +1570,64 @@ extern "C" int gdrn_bn_fwd(const void* x_hi, const void* x_lo, const void* r_hi,
         if (r_hi != nullptr) GDRN_BN_FWD(false, true); else GDRN_BN_FWD(false, false);
     }
 #undef GDRN_BN_FWD
+    LAUNCH_DONE();
+}
+
+static int check_head_gn(const char* fn, int B, int HW, int C, int G) {
+    if (C != kGnHeadC) return set_error(GDRN_ERR_ARG, "%s: C = %d (the geometry head's GroupNorm has C = 256)", fn, C);
+    if (G < 1 || G > 64 || kGnHeadC % G) return set_error(GDRN_ERR_ARG, "%s: G = %d (a divisor of 256, at most 64)", fn, G);
+    if (HW != 256 && HW != 1024 && HW != 4096) return set_error(GDRN_ERR_ARG, "%s: HW = %d (256, 1024 or 4096)", fn, HW);
+    if (B < 1) return set_error(GDRN_ERR_ARG, "%s: B = %d", fn, B);
+    return 0;
+}
+
+extern "C" long long gdrn_head_gn_workspace(int B, int HW) {
+    if (B < 1 || (HW != 256 && HW != 1024 && HW != 4096)) return -1;
+    return gn_head_ws_gred(B, gn_head_splits(HW)) + (long long)B * 64;
+}
+
+extern "C" int gdrn_head_gn_fwd(const void* u_hi, const void* u_lo, void* y_hi, void* y_lo, void* relu_mask_out, const float* gamma,
+                                const float* beta, float* stats, double* ws, int B, int HW, int C, int G, float eps, void* stream_) {
+    STREAM;
+    if (int rc = check_head_gn("head_gn_fwd", B, HW, C, G)) return rc;
+    if (!u_hi || !y_hi || !gamma || !beta || !stats || !ws)
+        return set_error(GDRN_ERR_ARG, "head_gn_fwd: u, y, gamma, beta, stats and the workspace are required");
+    const int S = gn_head_splits(HW);
+    gn_head_stats_partial_kernel<<<dim3(S, B), 256, 0, stream>>>(CBF(u_hi), CBF(u_lo), ws, HW, G);
+    GDRN_CUDA_OK(cudaGetLastError());
+    count_launch();
+    gn_head_stats_final_kernel<<<(B * G + 127) / 128, 128, 0, stream>>>(ws, stats, B, S, G, (double)HW * (kGnHeadC / G), eps);
+    GDRN_CUDA_OK(cudaGetLastError());
+    count_launch();
+    const long n8 = (long)B * HW * (kGnHeadC / 8);
+    gn_head_apply_kernel<<<ew_grid(n8, 256), 256, 0, stream>>>(CBF(u_hi), CBF(u_lo), BF(y_hi), BF(y_lo),
+                                                               reinterpret_cast<uint8_t*>(relu_mask_out), gamma, beta, stats, n8, HW, G);
+    LAUNCH_DONE();
+}
+
+extern "C" int gdrn_head_gn_bwd(const void* g_hi, const void* g_lo, const void* u_hi, const void* u_lo, const void* relu_mask,
+                                const float* gamma, const float* stats, void* du_hi, void* du_lo, float* dgamma, float* dbeta,
+                                double* ws, int B, int HW, int C, int G, void* stream_) {
+    STREAM;
+    if (int rc = check_head_gn("head_gn_bwd", B, HW, C, G)) return rc;
+    if (!g_hi || !u_hi || !relu_mask || !gamma || !stats || !du_hi || !dgamma || !dbeta || !ws)
+        return set_error(GDRN_ERR_ARG, "head_gn_bwd: g, u, the ReLU mask, gamma, stats, du, dgamma, dbeta and the workspace are required");
+    const int S = gn_head_splits(HW);
+    float* part = reinterpret_cast<float*>(ws);
+    double* crop = ws + gn_head_ws_crop(B, S);
+    float* gred = reinterpret_cast<float*>(ws + gn_head_ws_gred(B, S));
+    const uint8_t* mask = reinterpret_cast<const uint8_t*>(relu_mask);
+    gn_head_bwd_partial_kernel<<<dim3(S, B), 256, 0, stream>>>(CBF(g_hi), CBF(g_lo), CBF(u_hi), CBF(u_lo), mask, stats, part, HW, G);
+    GDRN_CUDA_OK(cudaGetLastError());
+    count_launch();
+    gn_head_bwd_crop_kernel<<<B, 256, 0, stream>>>(part, gamma, crop, gred, S, G, (double)HW * (kGnHeadC / G));
+    GDRN_CUDA_OK(cudaGetLastError());
+    count_launch();
+    gn_head_bwd_param_kernel<<<2, 256, 0, stream>>>(crop, dgamma, dbeta, B);
+    GDRN_CUDA_OK(cudaGetLastError());
+    count_launch();
+    const long n8 = (long)B * HW * (kGnHeadC / 8);
+    gn_head_bwd_apply_kernel<<<ew_grid(n8, 256), 256, 0, stream>>>(CBF(g_hi), CBF(g_lo), CBF(u_hi), CBF(u_lo), mask, gamma, stats,
+                                                                   gred, BF(du_hi), BF(du_lo), n8, HW, G);
     LAUNCH_DONE();
 }

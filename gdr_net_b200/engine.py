@@ -266,6 +266,12 @@ class Engine:
             self.loss_names = self.loss_names[5:]
         assert int(C.load().gdrn_pose_loss_count(self.pose_sw)) == len(pose_names), (sw, pose_names)
         self.named_params = list(model.named_parameters())
+        # geometry-head normalisation (ROT_HEAD.NORM): "GN" takes the head's seven norm layers out of the BatchNorm tables, the
+        # statistic slices and the fold jobs; they run the gdrn_head_gn_* kernels (no running statistics: train = eval)
+        self.head_gn = rh.NORM == "GN"
+        self._gn_mods = {n: m for n, m in model.rot_head_net.named_modules(prefix="rot_head_net")
+                         if isinstance(m, torch.nn.GroupNorm)} if self.head_gn else {}
+        self._last_gstats = None
         self.bn: Dict[str, _BN] = {}
         total = 0
         self._bn_mods = {}
@@ -422,8 +428,9 @@ class Engine:
                 out += [(p + ".conv1", p + ".bn1"), (p + ".conv2", p + ".bn2")]
                 if blk.downsample is not None:
                     out.append((p + ".downsample.0", p + ".downsample.1"))
-        out.append(("deconv", "rot_head_net.features.1"))
-        out += [(f"rot_head_net.features.{ci}", f"rot_head_net.features.{bi}") for ci, bi, _u in HEAD_CONVS]
+        if not self.head_gn:  # GroupNorm has no running statistics to fold
+            out.append(("deconv", "rot_head_net.features.1"))
+            out += [(f"rot_head_net.features.{ci}", f"rot_head_net.features.{bi}") for ci, bi, _u in HEAD_CONVS]
         return out
 
     def prepare_weights_folded(self):
@@ -481,6 +488,11 @@ class Engine:
         self._on_side(packs)
 
         def cbr(xin, ck, bk, conv, relu=True, res=None):
+            gn = self._gn_mods.get(bk)
+            if gn is not None:  # GroupNorm head: the unfolded conv, then GroupNorm + ReLU
+                u = (ops.conv_dgrad_s2(xin, self.wf[ck], conv.out_channels, 3, 1) if ck == "deconv"
+                     else ops.conv_fwd(xin, self.wf[ck], conv.out_channels, 3, 3, 1, 1))
+                return ops.head_gn_relu_fwd(u, gn.weight, gn.bias, gn.num_groups, gn.eps)[0]
             if ck == "deconv":
                 return ops.conv_dgrad_s2(xin, wfe[ck], conv.out_channels, 3, 1, bias=shift[bk], act=2 if relu else 0)
             k, stride, pad = conv.kernel_size[0], conv.stride[0], conv.padding[0]
@@ -654,12 +666,19 @@ class Engine:
         return self._det_ws
 
     def _conv_bn(self, x: PT, ckey: str, conv, bkey: str, relu: bool, train_bn: bool, res: Optional[PT] = None):
-        stats = self.bn[bkey].stats64 if (train_bn and not self.deterministic) else None  # deterministic: from gdrn_bn_stats
+        """conv -> BatchNorm or, in a GroupNorm head, GroupNorm (+ ReLU); a GroupNorm leaves its statistics in _last_gstats."""
+        gn = self._gn_mods.get(bkey)
+        # deterministic: from gdrn_bn_stats
+        stats = self.bn[bkey].stats64 if (gn is None and train_bn and not self.deterministic) else None
         k, stride, pad = conv.kernel_size[0], conv.stride[0], conv.padding[0]
         if ckey == "deconv":
             u = ops.conv_dgrad_s2(x, self.wf["deconv"], conv.out_channels, 3, 1, stats=stats)
         else:
             u = ops.conv_fwd(x, self.wf[ckey], conv.out_channels, k, k, stride, pad, stats=stats)
+        if gn is not None:
+            y, self._last_gstats, self._last_mask = ops.head_gn_relu_fwd(u, gn.weight, gn.bias, gn.num_groups, gn.eps,
+                                                                         want_mask=self._want_masks)
+            return u, y
         return u, self._bn_fwd(bkey, u, relu, train_bn, res)
 
     # ------------------------------------------------------------------------------------------ forward
@@ -763,7 +782,7 @@ class Engine:
         self._want_masks = keep_head
         u, y = self._conv_bn(feat, "deconv", hf[0], "rot_head_net.features.1", True, train_bn)
         if keep_head:
-            S["deconv"] = dict(z=feat, u=u, y=y, m=self._last_mask)
+            S["deconv"] = dict(z=feat, u=u, y=y, m=self._last_mask, gs=self._last_gstats)
             S["head"] = []
         cur = y
         for ci, bi, up in HEAD_CONVS:
@@ -771,7 +790,7 @@ class Engine:
                 cur = ops.upsample2x_fwd(cur)
             u, y = self._conv_bn(cur, f"rot_head_net.features.{ci}", hf[ci], f"rot_head_net.features.{bi}", True, train_bn)
             if keep_head:
-                S["head"].append(dict(ci=ci, bi=bi, up=up, x_in=cur, u=u, y=y, m=self._last_mask))
+                S["head"].append(dict(ci=ci, bi=bi, up=up, x_in=cur, u=u, y=y, m=self._last_mask, gs=self._last_gstats))
             cur = y
         head_in = cur  # [B,64,64,256]
         if self._nbt:
@@ -906,6 +925,13 @@ class Engine:
                           beta=mod.bias, sums_zeroed=True, relu_mask=mask,
                           det_ws=self._det_workspace() if self.deterministic else None)
 
+    def _head_norm_bwd(self, bkey: str, g: PT, u: PT, L: dict) -> PT:
+        """Backward of a head norm layer + ReLU (L: its saved forward entry) -> the gradient of its conv output."""
+        gn = self._gn_mods.get(bkey)
+        if gn is None:
+            return self._bn_bwd(bkey, g, None, u, mask=L["m"])[0]
+        return ops.head_gn_relu_bwd(g, u, L["m"], gn.weight, L["gs"], self.grads[bkey + ".weight"], self.grads[bkey + ".bias"])
+
     def backward(self, grad_losses: torch.Tensor):
         """grad_losses: upstream gradients of self.loss_names ([8], LOSS_NAMES, by default).  Fills self.grads (views of
         self.flat_grad)."""
@@ -1001,13 +1027,13 @@ class Engine:
         # ---- head convs (cdpn_rot_head_region.py:95-125)
         for L in reversed(S["head"]):
             ci, bi = L["ci"], L["bi"]
-            du, _ = self._bn_bwd(f"rot_head_net.features.{bi}", g, None, h(L["u"]), mask=L["m"])
+            du = self._head_norm_bwd(f"rot_head_net.features.{bi}", g, h(L["u"]), L)
             self._wgrad_conv(du, h(L["x_in"]), hf[ci], f"rot_head_net.features.{ci}.weight")
             g = self._dgrad_conv(du, hf[ci], f"rot_head_net.features.{ci}")
             if L["up"]:
                 g = ops.upsample2x_bwd(g)
         D = S["deconv"]
-        du, _ = self._bn_bwd("rot_head_net.features.1", g, None, h(D["u"]), mask=D["m"])
+        du = self._head_norm_bwd("rot_head_net.features.1", g, h(D["u"]), D)
         def deconv_wgrad(du=du):
             # d wt[ci][co][r][s] = sum_q x[ci][q] * du[co][2q + (r, s) - 1]: the weight gradient of the stride-2 conv du -> x
             # with x in the role of dY; its [O = 512][I = 256][3][3] layout IS the ConvTranspose2d IOHW layout (no flip)

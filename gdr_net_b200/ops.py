@@ -421,6 +421,33 @@ def gn_relu_bwd(g: PT, y: PT, u: PT, gamma, stats, dgamma, dbeta, G=32) -> PT:
     return du
 
 
+def head_gn_workspace(B: int, HW: int, dev) -> torch.Tensor:
+    """Scratch of gdrn_head_gn_fwd / _bwd (float64): the partial sums of their two-stage reductions."""
+    return torch.empty(int(C.load().gdrn_head_gn_workspace(B, HW)), dtype=torch.float64, device=dev)
+
+
+def head_gn_relu_fwd(u: PT, gamma, beta, G: int, eps: float = 1e-5, want_mask: bool = False):
+    """Geometry-head GroupNorm(G, 256) + ReLU: (y, stats [B, G, 2] = (mean, invstd), ReLU bitmap or None)."""
+    B, H, W, Cc = u.shape
+    out = like(u)
+    stats = torch.empty(B, G, 2, device=u.buf.device)
+    mask = torch.empty(u.numel() // 8, dtype=torch.uint8, device=u.buf.device) if want_mask else None
+    ws = head_gn_workspace(B, H * W, u.buf.device)
+    C.gdrn_head_gn_fwd(u.hi_ptr, u.lo_ptr, out.hi_ptr, out.lo_ptr, ptr(mask), gamma.data_ptr(), beta.data_ptr(), stats.data_ptr(),
+                       ws.data_ptr(), B, H * W, Cc, G, float(eps), _stream())
+    return out, stats, mask
+
+
+def head_gn_relu_bwd(g: PT, u: PT, mask, gamma, stats, dgamma, dbeta) -> PT:
+    """Backward of head_gn_relu_fwd: dL/du in g's planes; dgamma / dbeta are written, not accumulated."""
+    B, H, W, Cc = u.shape
+    du = like(g)
+    ws = head_gn_workspace(B, H * W, g.buf.device)
+    C.gdrn_head_gn_bwd(g.hi_ptr, g.lo_ptr, u.hi_ptr, u.lo_ptr, mask.data_ptr(), gamma.data_ptr(), stats.data_ptr(), du.hi_ptr, du.lo_ptr,
+                       dgamma.data_ptr(), dbeta.data_ptr(), ws.data_ptr(), B, H * W, Cc, stats.shape[1], _stream())
+    return du
+
+
 def add2(a: PT, b: PT) -> PT:
     out = like(a)
     C.gdrn_add2(a.hi_ptr, a.lo_ptr, b.hi_ptr, b.lo_ptr, out.hi_ptr, out.lo_ptr, a.numel(), _stream())

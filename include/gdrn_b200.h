@@ -157,6 +157,19 @@ int gdrn_gn_relu_fwd(const void* u_hi, const void* u_lo, void* y_hi, void* y_lo,
 int gdrn_gn_relu_bwd(const void* g_hi, const void* g_lo, const void* y_hi, const void* u_hi, const void* u_lo,
                      const float* gamma, const float* stats, void* du_hi, void* du_lo, float* dgamma, float* dbeta, int B,
                      int HW, int C, int G, void* stream);
+/* ---- GroupNorm(G, 256) + ReLU of the geometry head (ROT_HEAD.NORM = "GN", NUM_GN_GROUPS = G; cdpn_rot_head_region.py with
+ * get_norm("GN")).  NHWC [B][HW][256] in 16-bit planes (lo = NULL: one plane), G | 256, G <= 64, HW in {256, 1024, 4096}.
+ * Two-stage reductions in a fixed order, no atomics: bit-identical results run to run.
+ * ws: gdrn_head_gn_workspace(B, HW) doubles (-1 for unsupported arguments).
+ * fwd: stats [B][G][2] = (mean, invstd); y = relu(gamma (u - mean) invstd + beta); relu_mask_out (optional) [B*HW*32] bytes,
+ *      bit j of byte i = y[8 i + j] > 0 (the gdrn_bn_fwd bitmap).
+ * bwd: g is dL/dy, relu_mask the forward's bitmap; du = dL/du; dgamma / dbeta are written (not accumulated). */
+long long gdrn_head_gn_workspace(int B, int HW);
+int gdrn_head_gn_fwd(const void* u_hi, const void* u_lo, void* y_hi, void* y_lo, void* relu_mask_out, const float* gamma,
+                     const float* beta, float* stats, double* ws, int B, int HW, int C, int G, float eps, void* stream);
+int gdrn_head_gn_bwd(const void* g_hi, const void* g_lo, const void* u_hi, const void* u_lo, const void* relu_mask,
+                     const float* gamma, const float* stats, void* du_hi, void* du_lo, float* dgamma, float* dbeta, double* ws,
+                     int B, int HW, int C, int G, void* stream);
 int gdrn_add2(const void* a_hi, const void* a_lo, const void* b_hi, const void* b_lo, void* o_hi, void* o_lo, long n,
               void* stream);
 /* bias gradients (column sums of a [rows][ld] planar tensor) and LeakyReLU(0.1) backward (conv_pnp_net.py:93,152-153) */
