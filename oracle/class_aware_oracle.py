@@ -30,8 +30,8 @@ def select_class_maps(head: Tensor, classes: Tensor, num_classes: int, mo: int, 
     mask = head[:, :mo * cm].reshape(B, cm, mo, H, W)
     xyz = head[:, mo * cm:mo * cm + 3 * cr].reshape(B, 3, cr, H, W)
     region = head[:, mo * cm + 3 * cr:].reshape(B, cg, R + 1, H, W)
-    b = torch.arange(B)
-    cls = classes.long()
+    b = torch.arange(B, device=head.device)
+    cls = classes.long().to(head.device)
     zero = torch.zeros_like(cls)
     mask = mask[b, cls if mask_aware else zero]                                     # [B, MO, H, W]
     xyz = xyz[b, :, cls if rot_aware else zero]                                     # [B, 3, H, W]

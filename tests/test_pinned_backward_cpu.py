@@ -5,8 +5,16 @@
     codes).  Replayed through the shim, every pin is consumed, no decision differs and the gradients and running statistics
     equal plain autograd's.
   * The decoders against hand-built cases: bit order, max-pool ties, border windows, codes that point into the padding.
+  * The same at B = 2 for every other replay path (BCE / CE mask heads, the pose-loss switches with Smooth-L1, L2, MSE and
+    symmetric point matching, a class-aware head, the GroupNorm head, DropBlock, a frozen backbone and Patch-PnP): every pin
+    kind is consumed, no decision differs, and the gradients equal plain autograd's.  For the pose switches the loss pins are
+    also built the way `capture` builds them, from fp32 outputs in the engine's layouts, and must agree with the oracle's own.
+  * Hand-built Smooth-L1 residuals at |d| = beta and symmetric candidates that tie.
   * The comparator flags a planted 1 % error in one row of a 512-row tensor, which a tensor-level rel-L2 would not notice.
 """
+import math
+import types
+
 import numpy as np
 import pytest
 import torch
@@ -14,8 +22,17 @@ import torch.nn.functional as TF
 
 import pinned_backward as PB
 from gdr_net_b200 import synth
+from oracle import class_aware_oracle as CA
+from oracle import dropblock_oracle as DB
 from oracle import fixtures
+from oracle import freeze_oracle as FO
 from oracle import gdrn_oracle as O
+from oracle import head_gn_oracle as HG
+from oracle import mask_oracle as M
+from oracle import pose_loss_oracle as P
+from oracle import region_oracle as RO
+import test_class_aware_cpu as TCA  # noqa: E402 (tests/ is on sys.path)
+import test_pose_losses_cpu as TPL  # noqa: E402
 
 
 # ------------------------------------------------------------------------------------------------ independent encoder
@@ -44,7 +61,8 @@ def encode_pool(x_nchw: torch.Tensor) -> torch.Tensor:
 
 
 class Recorder:
-    """torch.nn.functional with the arguments of the decision calls recorded in call order."""
+    """torch.nn.functional with the arguments of the decision calls recorded in call order (calls without gradient, which
+    decide nothing, are not recorded)."""
 
     def __init__(self):
         self.calls = []
@@ -53,15 +71,22 @@ class Recorder:
         return getattr(TF, name)
 
     def relu(self, x, inplace=False):
-        self.calls.append(("relu", x.detach().clone()))
+        if x.requires_grad:
+            self.calls.append(("relu", x.detach().clone()))
         return TF.relu(x)
 
     def leaky_relu(self, x, negative_slope=0.01, inplace=False):
         self.calls.append(("leaky_relu", x.detach().clone()))
         return TF.leaky_relu(x, negative_slope)
 
+    def linear(self, x, weight, bias=None):
+        y = TF.linear(x, weight, bias)
+        self.calls.append(("linear", (tuple(x.shape), y.detach().clone())))
+        return y
+
     def max_pool2d(self, x, *a, **k):
-        self.calls.append(("max_pool2d", x.detach().clone()))
+        if x.requires_grad:
+            self.calls.append(("max_pool2d", x.detach().clone()))
         return TF.max_pool2d(x, *a, **k)
 
     def l1_loss(self, a, b, reduction="mean", **k):
@@ -69,14 +94,23 @@ class Recorder:
             self.calls.append(("l1_loss", (a - b).detach().clone()))
         return TF.l1_loss(a, b, reduction=reduction)
 
+    def smooth_l1_loss(self, a, b, reduction="mean", beta=1.0, **k):
+        self.calls.append(("smooth_l1_loss", ((a - b).detach().clone(), beta)))
+        return TF.smooth_l1_loss(a, b, reduction=reduction, beta=beta)
 
-def pins_from_oracle(calls):
-    """Pins in the engine's layouts from recorded oracle calls: BatchNorm sites as bitmaps, GroupNorm (the three ReLUs after the
-    40 BatchNorm ones) and LeakyReLU sites from their outputs, the max-pool as codes, the L1 calls as signs."""
+    def closest_rot_batch(self, pred_rots, gt_rots, sym_infos):
+        self.calls.append(("closest_rot_batch", PB.closest_sym_index(pred_rots, gt_rots, sym_infos)))
+        return O.closest_rot_batch(pred_rots, gt_rots, sym_infos)
+
+
+def pins_from_oracle(calls, n_bitmaps=40):
+    """Pins in the engine's layouts from recorded oracle calls: BatchNorm / head-norm sites (the first n_bitmaps ReLUs) as
+    bitmaps, the Patch-PnP GroupNorm and LeakyReLU sites from their outputs, the max-pool as codes, the L1 calls as signs, the
+    Smooth-L1 calls as branch / sign codes, the symmetric search as candidate indices."""
     pins, n_relu = [], 0
     for i, (kind, x) in enumerate(calls):
         name = f"{kind}#{i}"
-        if kind == "relu" and n_relu < 40:
+        if kind == "relu" and n_relu < n_bitmaps:
             B, C, H, W = x.shape
             pins.append(PB.Pin.relu_bitmap(name, encode_bitmap(x), (B, H, W, C)))
         elif kind == "relu":
@@ -86,10 +120,57 @@ def pins_from_oracle(calls):
         elif kind == "max_pool2d":
             B, C, H, W = x.shape
             pins.append(PB.Pin.pool(name, encode_pool(x), (B, H, W, C)))
+        elif kind == "linear":  # the rotation / translation outputs (6 and 3 wide) as values, fc1 and fc2 unpinned
+            pins.append(PB.Pin.linear(name, x[0], x[1] if x[1].shape[1] <= 6 else None))
+        elif kind == "smooth_l1_loss":
+            pins.append(PB.Pin.smooth_l1(name, x[0], x[1]))
+        elif kind == "closest_rot_batch":
+            pins.append(PB.Pin.sym(name, x))
         else:
             pins.append(PB.Pin.sign(name, torch.sign(x)))
         n_relu += kind == "relu"
     return pins
+
+
+def record(fwd, sd, batch, modules):
+    """The plain float64 step with the decision calls recorded: (calls, result, leaf state dict)."""
+    rec = Recorder()
+    old = [(m, m.F) for m in modules]
+    for m in modules:
+        m.F = rec
+    try:
+        out, leaf, _ = PB.replay(fwd, sd, batch, None, modules, device="cpu")
+    finally:
+        for m, f in old:
+            m.F = f
+    return rec.calls, out, leaf
+
+
+def assert_replay_is_autograd(sd, batch, fwd, modules, pins, out, leaf, inert=0):
+    """The pinned replay consumes every pin, decides nothing differently and gives plain autograd's losses, gradients and
+    running statistics."""
+    out_p, leaf_p, shim = PB.replay(fwd, sd, batch, pins, modules, device="cpu")
+    assert len(shim.sites) == len(pins) and shim.inert == inert, (len(shim.sites), len(pins), shim.inert)
+    assert all(s["flips"] == 0 for s in shim.sites), [s for s in shim.sites if s["flips"]]
+    assert list(out_p["losses"]) == list(out["losses"])
+    for k, v in out["losses"].items():
+        assert abs(float(out_p["losses"][k].detach()) - float(v.detach())) <= 1e-12 * abs(float(v)), k
+    worst, worst_rel = 0.0, 0.0
+    for name, t in leaf.items():
+        if isinstance(t, torch.Tensor) and t.requires_grad:
+            assert (leaf_p[name].grad is None) == (t.grad is None), name
+            if t.grad is None:
+                continue
+            e, rel = PB.row_errors(leaf_p[name].grad, t.grad)
+            worst, worst_rel = max(worst, float(e.max())), max(worst_rel, rel)
+        elif name.endswith(("running_mean", "running_var")):
+            assert float((leaf_p[name] - t).abs().max()) <= 1e-12 * float(t.abs().max()), name
+        elif name.endswith("num_batches_tracked"):
+            assert int(leaf_p[name]) == int(t) == int(sd[name]) + 1, name
+    # measured: rel-L2 <= 4e-13 per tensor; rows whose gradient is a cancelling sum (BatchNorm, GroupNorm entries) reach 5e-10
+    print(f"pinned vs plain autograd, float64 B = 2: worst rel-L2 {worst_rel:.1e}, worst per-row error {worst:.1e}")
+    assert worst_rel < 2e-12 and worst < 1e-8
+    return shim
 
 
 @pytest.fixture(scope="module")
@@ -97,20 +178,17 @@ def oracle_b2():
     sd = fixtures.calibrated_state_dict(0)
     batch = synth.make_batch(2, seed=3)
     fwd = lambda leaf, b: O.gdrn_forward(leaf, b, train=True, do_loss=True, update_stats=True)  # noqa: E731
-    rec = Recorder()
-    old = O.F
-    O.F = rec
-    try:
-        out, leaf, _ = PB.replay(fwd, sd, batch, None, (O,), device="cpu")
-    finally:
-        O.F = old
-    return sd, batch, fwd, rec.calls, out, leaf
+    calls, out, leaf = record(fwd, sd, batch, (O,))
+    return sd, batch, fwd, calls, out, leaf
 
 
 def test_recorded_call_order_is_the_engines(oracle_b2):
     calls = oracle_b2[3]
     kinds = [k for k, _ in calls]
-    assert kinds == ["relu", "max_pool2d"] + ["relu"] * 39 + ["relu"] * 3 + ["leaky_relu"] * 2 + ["l1_loss"] * 7
+    assert kinds == (["relu", "max_pool2d"] + ["relu"] * 39 + ["relu"] * 3 + ["linear", "leaky_relu"] * 2 + ["linear"] * 2
+                     + ["l1_loss"] * 7)
+    assert [x[1].shape for k, x in calls if k == "linear"] == [(2, 1024), (2, 256), (2, 6), (2, 3)]
+    calls = [c for c in calls if c[0] != "linear"]
     shapes = [tuple(x.shape) for _, x in calls]
     assert shapes[0] == (2, 64, 128, 128) and shapes[1] == (2, 64, 128, 128) and shapes[40] == (2, 256, 64, 64) and shapes[41] == (2, 128, 32, 32)
     assert shapes[-7:-3] == [(2, 1, 64, 64)] * 3 + [(2, 64, 64)] and shapes[-2:] == [(2, 2), (2,)]
@@ -121,24 +199,8 @@ def test_pinned_replay_equals_autograd(oracle_b2):
     """Pins from the oracle's own decisions: the pinned float64 step is the plain one, to rounding."""
     sd, batch, fwd, calls, out, leaf = oracle_b2
     pins = pins_from_oracle(calls)
-    assert len(pins) == 53
-    out_p, leaf_p, shim = PB.replay(fwd, sd, batch, pins, (O,), device="cpu")
-    assert len(shim.sites) == 53 and shim.inert == 0
-    assert all(s["flips"] == 0 for s in shim.sites), [s for s in shim.sites if s["flips"]]
-    for k, v in out["losses"].items():
-        assert abs(float(out_p["losses"][k].detach()) - float(v.detach())) <= 1e-12 * abs(float(v)), k
-    worst, worst_rel = 0.0, 0.0
-    for name, t in leaf.items():
-        if isinstance(t, torch.Tensor) and t.requires_grad:
-            e, rel = PB.row_errors(leaf_p[name].grad, t.grad)
-            worst, worst_rel = max(worst, float(e.max())), max(worst_rel, rel)
-        elif name.endswith(("running_mean", "running_var")):
-            assert float((leaf_p[name] - t).abs().max()) <= 1e-12 * float(t.abs().max()), name
-        elif name.endswith("num_batches_tracked"):
-            assert int(leaf_p[name]) == int(t) == int(sd[name]) + 1, name
-    # measured: rel-L2 <= 4e-13 per tensor; rows whose gradient is a cancelling sum (BatchNorm, GroupNorm entries) reach 5e-10
-    print(f"pinned vs plain autograd, float64 B = 2: worst rel-L2 {worst_rel:.1e}, worst per-row error {worst:.1e}")
-    assert worst_rel < 2e-12 and worst < 1e-8
+    assert len(pins) == 57
+    assert_replay_is_autograd(sd, batch, fwd, (O,), pins, out, leaf)
 
 
 def test_every_pin_must_be_consumed_and_match(oracle_b2):
@@ -161,6 +223,212 @@ def test_flipped_decisions_are_counted(oracle_b2):
     pins[2] = PB.Pin.relu_bitmap("flipped", inv, (B, H, W, C))
     _, _, shim = PB.replay(fwd, sd, batch, pins, (O,), device="cpu", parity=False)
     assert shim.sites[2]["flips"] == B * C * H * W // 8
+
+
+# ------------------------------------------------------------------------------------------------ the other replay paths
+def _seeded(rot_head=None, pnp_net=None, seed=0):
+    """Seeded weights (synth.seeded_state_dict) of the model build_model_optimizer makes with these switches."""
+    from gdr_net_b200 import GDRN as G
+    from gdr_net_b200.config import a6_config
+
+    cfg = a6_config(device="cpu")
+    for k, v in (rot_head or {}).items():
+        setattr(cfg.MODEL.CDPN.ROT_HEAD, k, v)
+    for k, v in (pnp_net or {}).items():
+        setattr(cfg.MODEL.CDPN.PNP_NET, k, v)
+    model, _ = G.build_model_optimizer(cfg)
+    return synth.seeded_state_dict(model.state_dict(), seed=seed), cfg
+
+
+def _sym_batch():
+    """Two crops whose objects are symmetric: a four-fold and a discretised continuous axis."""
+    batch = synth.make_batch(2, seed=3)
+    batch["sym_info"] = [synth.discrete_symmetries("z4"), synth.discrete_symmetries("cont")]
+    return batch
+
+
+POSE = {k: TPL.CASES[k][0] for k in ("rt_sl1", "disz_l2", "dist_nop_sym")}
+POSE["rt_l1_trans"] = dict(PM_R_ONLY=False, PM_DISENTANGLE_T=True, PM_T_USE_POINTS=True, PM_LOSS_TYPE="L1", TRANS_LW=1.0,
+                           TRANS_LOSS_TYPE="L1", TRANS_LOSS_DISENTANGLE=False)  # L1 point matching with points, L1 translation
+
+
+def _path(name):
+    """(state dict, batch, forward, oracle modules, bitmap sites, inert calls, pose config or None) of one replay path."""
+    sd0 = fixtures.calibrated_state_dict(0)
+    batch = synth.make_batch(2, seed=3)
+    if name in ("bce", "ce"):
+        kind = name.upper()
+        sd = _seeded({"MASK_LOSS_TYPE": "CE"}, seed=6)[0] if kind == "CE" else sd0
+        gt = ("obj", "visib", "visib") if kind == "BCE" else ("visib", "obj", "trunc")  # test_mask_heads_cpu.CASES
+        fwd = lambda leaf, b: M.gdrn_forward(leaf, b, True, True, mask_loss_type=kind, mask_gt=gt, update_stats=True)  # noqa: E731
+        return sd, batch, fwd, (O, M), 40, 4, None
+    if name in POSE:
+        p = TPL.pose_config(**POSE[name]).MODEL.CDPN.PNP_NET
+        sym = bool(POSE[name].get("PM_LOSS_SYM"))
+        fwd = lambda leaf, b: P.gdrn_forward(leaf, b, p, train=True, pm_sym=sym, update_stats=True)  # noqa: E731
+        return sd0, (_sym_batch() if sym else batch), fwd, (O, M, P), 40, 4, p
+    if name == "all13":
+        sd = _seeded(dict(NUM_CLASSES=13, ROT_CLASS_AWARE=True, MASK_CLASS_AWARE=True, REGION_CLASS_AWARE=True), seed=51)[0]
+        batch["roi_cls"] = torch.tensor([3, 12])
+        kw = dict(num_classes=13, rot_aware=True, mask_aware=True, region_aware=True, num_regions=64)
+        fwd = lambda leaf, b: CA.gdrn_forward(leaf, b, True, True, update_stats=True, **kw)  # noqa: E731
+        return sd, batch, fwd, (O, M, RO), 40, 4, None
+    if name == "mr_ce21":  # CE mask head, class-aware mask and region blocks, 8 regions
+        sd = TCA.seeded_weights(name)
+        batch = synth.make_batch(2, seed=3, num_regions=8)
+        batch["roi_cls"] = torch.tensor([5, 20])
+        kw = TCA.oracle_kwargs(name)
+        fwd = lambda leaf, b: CA.gdrn_forward(leaf, b, True, True, update_stats=True, **kw)  # noqa: E731
+        return sd, batch, fwd, (O, M, RO), 40, 4, None
+    if name == "gn":
+        sd = _seeded(dict(NORM="GN", NUM_GN_GROUPS=32), seed=71)[0]
+        fwd = lambda leaf, b: HG.gdrn_forward(leaf, b, True, True, G=32, update_stats=True)  # noqa: E731
+        return sd, batch, fwd, (O, M, RO, HG), 40, 4, None
+    if name == "dropblock":
+        seeds = (torch.rand(2, 64, 64, generator=torch.Generator().manual_seed(5)) < 0.25 / 25).float()
+        fwd = lambda leaf, b: DB.gdrn_forward(leaf, b, True, True, seeds=seeds, block_size=5, update_stats=True)  # noqa: E731
+        return sd0, batch, fwd, (O, M, RO, DB), 40, 5, None  # + DropBlock's max-pool over the seed mask
+    if name == "bb_pnp":
+        fwd = lambda leaf, b: FO.gdrn_forward(leaf, b, True, True, freeze=FO.CASES["bb_pnp"], update_stats=True)  # noqa: E731
+        return sd0, batch, fwd, (O,), 7, 33 + 1, None  # the frozen backbone's 33 ReLUs and its max-pool
+    raise KeyError(name)
+
+
+PATHS = ["bce", "ce", "rt_sl1", "disz_l2", "dist_nop_sym", "rt_l1_trans", "all13", "mr_ce21", "gn", "dropblock", "bb_pnp"]
+LOSS_KINDS = {  # the decision calls of the loss terms, in order (the shipped pose terms that pose_loss_oracle drops included)
+    "bce": ["l1_loss"] * 3 + ["l1_loss"] * 3,
+    "ce": ["l1_loss"] * 3 + ["l1_loss"] * 3,
+    "mr_ce21": ["l1_loss"] * 3 + ["l1_loss"] * 3,
+    "rt_sl1": ["l1_loss"] * 7 + ["smooth_l1_loss", "l1_loss", "l1_loss", "l1_loss"],      # PM_RT, centroid, z, bind
+    "disz_l2": ["l1_loss"] * 7,                                                               # all smooth
+    "dist_nop_sym": ["l1_loss"] * 7 + ["closest_rot_batch", "l1_loss", "l1_loss", "l1_loss"],  # centroid, z, bind
+    "rt_l1_trans": ["l1_loss"] * 7 + ["l1_loss"] * 5,                                        # PM_R, PM_T, centroid, z, LPnP
+}
+
+
+@pytest.mark.parametrize("name", PATHS)
+def test_every_replay_path_equals_autograd(name):
+    sd, batch, fwd, modules, n_bitmaps, inert, _ = _path(name)
+    calls, out, leaf = record(fwd, sd, batch, modules)
+    kinds = [k for k, _ in calls]
+    assert kinds.count("relu") == n_bitmaps + 3 and kinds.count("max_pool2d") == (n_bitmaps == 40)
+    if name in LOSS_KINDS:
+        assert kinds[n_bitmaps + 10:] == LOSS_KINDS[name], kinds[n_bitmaps + 10:]
+    if name == "dist_nop_sym":
+        idx = [x for k, x in calls if k == "closest_rot_batch"][0]
+        assert (idx >= 0).any(), idx  # a symmetric candidate is taken
+    if name == "rt_sl1":
+        d, beta = [x for k, x in calls if k == "smooth_l1_loss"][0]
+        inner = (d.abs() < beta).float().mean()
+        assert 0 < inner < 1, inner  # both branches are exercised
+    shim = assert_replay_is_autograd(sd, batch, fwd, modules, pins_from_oracle(calls, n_bitmaps), out, leaf, inert)
+    if name == "bb_pnp":
+        for k, t in leaf.items():
+            if isinstance(t, torch.Tensor) and t.requires_grad:
+                assert (t.grad is not None) == FO.live(k, FO.CASES["bb_pnp"]), k
+    assert {s["kind"] for s in shim.sites} >= set(kinds)
+
+
+def _engine_like(out, batch, p):
+    """An object with the attributes loss_sign_pins reads, holding the oracle's outputs in fp32 and the engine's layouts."""
+    B = batch["roi_img"].shape[0]
+    head = out["head"].detach().float()
+    logits = torch.zeros(B, 64, 64, 72)
+    logits[..., :head.shape[1]] = head.permute(0, 2, 3, 1)
+    pred = torch.zeros(B, 16)
+    pred[:, :6], pred[:, 6:9] = out["rot6d"].detach().float(), out["pred_t_"].detach().float()
+    f = lambda k: batch[k].float()  # noqa: E731
+    aux = dict(gt_mask_visib=f("roi_mask_visib"), gt_mask_trunc=f("roi_mask_trunc"), gt_mask_obj=f("roi_mask_obj"),
+               gt_xyz=f("roi_xyz"), gt_ego_rot=f("ego_rot"), gt_points=f("roi_points"), roi_extents=f("roi_extent"),
+               gt_trans=f("trans"), gt_trans_ratio=f("roi_trans_ratio"))
+    table = torch.zeros(0, 3, 3)
+    if p is not None and p.PM_LOSS_SYM:
+        sets = batch["sym_info"]
+        counts = [0 if s is None else s.shape[0] for s in sets]
+        table = torch.cat([s for s in sets if s is not None])
+        aux["sym_idx"] = torch.tensor([[sum(counts[:b]), counts[b]] for b in range(B)], dtype=torch.int32)
+    S = dict(B=B, aux=aux, logits=logits.view(-1, 72), out_rot=out["rot"].detach().float(), out_trans=out["trans"].detach().float(),
+             pred=pred)
+    cfg = types.SimpleNamespace(MODEL=types.SimpleNamespace(CDPN=types.SimpleNamespace(PNP_NET=p)))
+    return types.SimpleNamespace(saved=S, mask_out=1, mask_loss=0, mask_gt=M.DEFAULT_MASK_GT, live_head=True, pose_ex=p is not None,
+                                 model=types.SimpleNamespace(cfg=cfg, pnp_net=types.SimpleNamespace(fc_r=types.SimpleNamespace(out_features=6))),
+                                 sym_table=types.SimpleNamespace(table=table))
+
+
+@pytest.mark.parametrize("name", [n for n in PATHS if n in POSE])
+def test_loss_pins_from_fp32_outputs_agree_with_the_oracle(name):
+    """The loss pins `capture` forms from the engine's fp32 outputs (loss_sign_pins, pose_pins, sym_choice) follow the pose
+    oracle's call order and shapes and take its decisions: replayed with the network's pins from the oracle, every pin is
+    consumed, nothing flips and the gradients are plain autograd's."""
+    sd, batch, fwd, modules, n_bitmaps, inert, p = _path(name)
+    calls, out, leaf = record(fwd, sd, batch, modules)
+    n_net = sum(k in ("relu", "max_pool2d", "leaky_relu", "linear") for k, _ in calls)
+    eng = _engine_like(out, batch, p)
+    loss_pins = PB.loss_sign_pins(eng, eng.saved)
+    assert [q.kind for q in loss_pins] == [k for k, _ in calls[n_net:]]
+    assert_replay_is_autograd(sd, batch, fwd, modules, pins_from_oracle(calls, n_bitmaps)[:n_net] + loss_pins, out, leaf, inert)
+
+
+def test_capture_refuses_switches_without_a_pin():
+    from gdr_net_b200.config import a6_config
+
+    cfg = a6_config(device="cpu")
+    cfg.MODEL.CDPN.PNP_NET.PM_LOSS_TYPE, cfg.MODEL.CDPN.PNP_NET.PM_SMOOTH_L1_BETA = "Smooth_L1", 1e-6
+    eng = types.SimpleNamespace(saved=dict(aux={}), pose_ex=True, model=types.SimpleNamespace(cfg=cfg))
+    with pytest.raises(NotImplementedError, match="beta"):
+        PB.capture(eng)
+    eng = types.SimpleNamespace(saved=dict(aux=dict(sym_idx=torch.zeros(2, 2))), pose_ex=False, model=types.SimpleNamespace(cfg=a6_config(device="cpu")))
+    with pytest.raises(NotImplementedError, match="symmetric"):
+        PB.capture(eng)
+
+
+# ------------------------------------------------------------------------------------------------ pin kinds, hand-built
+def test_smooth_l1_branch_at_beta():
+    """|d| = beta is the linear branch for the kernel and torch (|d| < beta is quadratic); both branches give the same value
+    and gradient there, so a pin taking the other branch is counted but changes nothing."""
+    beta = 0.5
+    d = torch.tensor([0.5, -0.5, 0.25, -1.5, 0.0, 0.4999999], dtype=torch.float64)
+    q = PB.Pin.smooth_l1("sl1", d, beta).decide("cpu")
+    assert q.tolist() == [1.0, -1.0, 0.0, -1.0, 0.0, 0.0]
+    for pin, flips in ((PB.Pin.smooth_l1("sl1", d, beta), 0), (PB.Pin.smooth_l1("wide", d, 0.6), 2)):
+        a = d.clone().requires_grad_(True)
+        shim = PB.PinnedF([pin])
+        v = shim.smooth_l1_loss(a, torch.zeros_like(d), reduction="mean", beta=beta)
+        v.backward()
+        b = d.clone().requires_grad_(True)
+        ref = TF.smooth_l1_loss(b, torch.zeros_like(d), reduction="mean", beta=beta)
+        ref.backward()
+        assert abs(float(v) - float(ref)) <= 1e-16 and torch.allclose(a.grad, b.grad, rtol=0, atol=1e-16), (pin.name, a.grad, b.grad)
+        assert shim.sites[0]["flips"] == flips
+        shim.finish()
+
+
+def _rz(a):
+    c, s = math.cos(a), math.sin(a)
+    return torch.tensor([[c, -s, 0.0], [s, c, 0.0], [0.0, 0.0, 1.0]], dtype=torch.float64)
+
+
+def test_symmetric_ties():
+    """A candidate that ties the unmodified R_gt loses to it; of two equal candidates the first is taken -- in the oracle's
+    float64 search, in the restatement of the pose kernel's fp32 one, and the shim follows its pin and counts a different
+    (equal-valued) choice as a flip."""
+    Rg = _rz(0.3) @ torch.tensor([[1.0, 0.0, 0.0], [0.0, 0.0, -1.0], [0.0, 1.0, 0.0]], dtype=torch.float64)
+    quarter = _rz(math.pi / 2)
+    sets = [torch.stack([torch.eye(3), _rz(math.pi)]).float(),          # crop 0: R = R_gt, identity candidate ties it
+            torch.stack([_rz(math.pi), quarter, quarter]).float()]      # crop 1: R = R_gt Rz(pi/2), candidates 1 and 2 tie
+    R = torch.stack([Rg, Rg @ quarter])
+    Rgs = torch.stack([Rg, Rg])
+    want = torch.tensor([-1, 1])
+    assert torch.equal(PB.closest_sym_index(R, Rgs, sets), want)
+    table = torch.cat(sets)
+    sym_idx = torch.tensor([[0, 2], [2, 3]], dtype=torch.int32)
+    assert torch.equal(PB.sym_choice(R.float(), Rgs.float(), table, sym_idx), want)
+    assert torch.allclose(O.closest_rot_batch(R, Rgs, sets), Rgs @ torch.stack([torch.eye(3, dtype=torch.float64), quarter]), rtol=0, atol=1e-7)
+    for pin_idx, flips in ((want, 0), (torch.tensor([-1, 2]), 1)):
+        shim = PB.PinnedF([PB.Pin.sym("sym", pin_idx)])
+        out = shim.closest_rot_batch(R, Rgs, sets)
+        assert torch.allclose(out, O.closest_rot_batch(R, Rgs, sets), rtol=0, atol=1e-7) and shim.sites[0]["flips"] == flips
+        shim.finish()
 
 
 # ------------------------------------------------------------------------------------------------ decoders, hand-built
@@ -260,3 +528,6 @@ def test_family_names():
     assert PB.family("rot_head_net.features.23.bias") == "rot_head_net/conv.bias"
     assert PB.family("pnp_net.features.4.bias") == "pnp_net/gn.bias"
     assert PB.family("pnp_net.fc_r.weight") == "pnp_net/fc.weight"
+    assert PB.family("rot_head_net.features.21.weight", head_gn=True) == "rot_head_net/gn.weight"
+    assert PB.family("rot_head_net.features.1.bias", head_gn=True) == "rot_head_net/gn.bias"
+    assert PB.family("rot_head_net.features.20.weight", head_gn=True) == "rot_head_net/conv.weight"
