@@ -92,21 +92,23 @@ class RotWithRegionHead(_ParamsOnly):
     """reference models/cdpn_rot_head_region.py:10-143 (ROT_CONCAT=False branch; concat mode is broken
     upstream, SURVEY P8).  `features` keeps the reference indices: ReLU / upsample placeholders included.
     With rot / mask / region_class_aware the output conv carries that block once per class (engine.class_rows).
-    norm = "BN" (nn.BatchNorm2d) or "GN" (nn.GroupNorm(num_gn_groups, 256), layer_utils.get_norm) at 1, 4, 7, 11, 14, 18, 21."""
+    norm = "BN" (nn.BatchNorm2d) or "GN" (nn.GroupNorm(num_gn_groups, 256), layer_utils.get_norm) at 1, 4, 7, 11, 14, 18, 21.
+    kernel_size = 2, 3 or 4: the stride-2 deconv at 0 (DECONV_PADDING), every one 8x8 -> 16x16; output_kernel_size = 1 or 3:
+    the output conv at 23 with padding k // 2 (cdpn_rot_head_region.py:33-46)."""
 
     def __init__(self, in_channels=512, num_layers=3, num_filters=256, kernel_size=3, output_kernel_size=1,
                  rot_output_dim=3, mask_output_dim=1, num_regions=64, norm="BN", num_gn_groups=32, freeze=False, num_classes=1,
                  rot_class_aware=False, mask_class_aware=False, region_class_aware=False):
         super().__init__()
         check_head_norm(norm, num_gn_groups)
-        if kernel_size != 3 or output_kernel_size != 1 or num_layers != 3:
-            raise NotImplementedError("only the a6 head (k3 deconv, 1x1 output conv, BN, 3 stages) is implemented")
+        check_head_shape(kernel_size, output_kernel_size, num_layers, num_filters)
         self.freeze = freeze
         f = nn.ModuleList()
         def norm_layer():
             return nn.GroupNorm(num_gn_groups, num_filters) if norm == "GN" else nn.BatchNorm2d(num_filters)
 
-        f.append(nn.ConvTranspose2d(in_channels, num_filters, 3, stride=2, padding=1, output_padding=1, bias=False))
+        pad, out_pad = DECONV_PADDING[kernel_size]
+        f.append(nn.ConvTranspose2d(in_channels, num_filters, kernel_size, stride=2, padding=pad, output_padding=out_pad, bias=False))
         f.append(norm_layer())
         f.append(nn.ReLU(inplace=True))
         for i in range(num_layers):
@@ -119,7 +121,8 @@ class RotWithRegionHead(_ParamsOnly):
         self.rot_output_dim = rot_output_dim * (num_classes if rot_class_aware else 1)
         self.mask_output_dim = mask_output_dim * (num_classes if mask_class_aware else 1)
         self.region_output_dim = (num_regions + 1) * (num_classes if region_class_aware else 1)
-        f.append(nn.Conv2d(num_filters, self.mask_output_dim + self.rot_output_dim + self.region_output_dim, 1, padding=0, bias=True))
+        f.append(nn.Conv2d(num_filters, self.mask_output_dim + self.rot_output_dim + self.region_output_dim, output_kernel_size,
+                           padding=output_kernel_size // 2, bias=True))
         self.features = f
         for m in self.modules():
             if isinstance(m, (nn.Conv2d, nn.ConvTranspose2d)):
@@ -127,6 +130,24 @@ class RotWithRegionHead(_ParamsOnly):
             elif isinstance(m, (nn.BatchNorm2d, nn.GroupNorm)):
                 nn.init.constant_(m.weight, 1.0)
                 nn.init.constant_(m.bias, 0.0)
+
+
+# ROT_HEAD.CONV_KERNEL_SIZE -> (padding, output_padding) of the head's stride-2 ConvTranspose2d (cdpn_rot_head_region.py:35-41)
+DECONV_PADDING = {2: (0, 0), 3: (1, 1), 4: (1, 0)}
+
+
+def check_head_shape(kernel_size, output_kernel_size, num_layers=3, num_filters=256):
+    """ROT_HEAD.CONV_KERNEL_SIZE (2, 3 or 4), OUT_CONV_KERNEL_SIZE (1 or 3), NUM_LAYERS (3: the 64x64 maps Patch-PnP's fc1 is
+    built for) and NUM_FILTERS (256, built into the head kernels and tables); anything else raises NotImplementedError naming
+    the key."""
+    if kernel_size not in DECONV_PADDING:
+        raise NotImplementedError(f"ROT_HEAD.CONV_KERNEL_SIZE = {kernel_size!r} (2, 3 or 4)")
+    if output_kernel_size not in (1, 3):
+        raise NotImplementedError(f"ROT_HEAD.OUT_CONV_KERNEL_SIZE = {output_kernel_size!r} (1 or 3)")
+    if num_layers != 3:
+        raise NotImplementedError(f"ROT_HEAD.NUM_LAYERS = {num_layers!r} (3)")
+    if num_filters != 256:
+        raise NotImplementedError(f"ROT_HEAD.NUM_FILTERS = {num_filters!r} (256)")
 
 
 def check_head_norm(norm, num_gn_groups):
@@ -247,6 +268,10 @@ def _check_supported(cfg):
         problems.append("concat heads (ROT_HEAD.ROT_CONCAT)")
     try:
         check_head_norm(r.NORM, r.get("NUM_GN_GROUPS", 32))
+    except NotImplementedError as e:
+        problems.append(str(e))
+    try:
+        check_head_shape(r.CONV_KERNEL_SIZE, r.OUT_CONV_KERNEL_SIZE, r.NUM_LAYERS, r.NUM_FILTERS)
     except NotImplementedError as e:
         problems.append(str(e))
     if (r.ROT_CLASS_AWARE or r.MASK_CLASS_AWARE or r.REGION_CLASS_AWARE) and not int(r.NUM_CLASSES) >= 1:

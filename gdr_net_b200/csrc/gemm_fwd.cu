@@ -617,10 +617,11 @@ extern "C" int gdrn_conv_fwd_grouped(const void* x_hi, const void* x_lo, const v
                          KW, stride, pad, ldc, act, nsplit, group, rows_per_group, num_groups, bias_stride, stream_);
 }
 
-// Data gradient of a stride-2 convolution (k = 3, pad 1 or k = 1, pad 0), decomposed by OUTPUT PARITY: the pixels
-// (2i + a, 2j + b) of dX only receive the filter taps r = a + pad (mod 2), so each of the four phases is a small stride-1
-// conv over the UN-dilated dY with 1 / 2 / 2 / 4 taps -- 9 taps per 4 output pixels instead of the 36 of the
-// "conv over zero-inserted dY" formulation, and no zero-inserted tensor in HBM.  One launch covers all phases.
+// Data gradient of a stride-2 convolution (k = 3, pad 1; k = 1, pad 0; k = 4, pad 1; k = 2, pad 0), decomposed by OUTPUT
+// PARITY: the pixels (2i + a, 2j + b) of dX only receive the filter taps r = a + pad (mod 2), so each of the four phases is a
+// small stride-1 conv over the UN-dilated dY -- k = 3: 1 / 2 / 2 / 4 taps, 9 taps per 4 output pixels instead of the 36 of the
+// "conv over zero-inserted dY" formulation; k = 4: 2x2 taps per phase; k = 2: one tap per phase -- and no zero-inserted tensor
+// in HBM.  One launch covers all phases.
 //   du [N][Ho][Wo][Cy] (Cy % 64 == 0), w = the dgrad-packed weights [Cx_pad][K*K*Cy] with flipped taps (pack_conv_dgrad),
 //   dx [N][2Ho][2Wo][ldc].  k = 1: only phase (0, 0) is computed, the caller passes a zero-filled dx.
 extern "C" int gdrn_conv_dgrad_s2(const void* du_hi, const void* du_lo, const void* w_hi, const void* w_lo, void* dx_hi,
@@ -629,7 +630,8 @@ extern "C" int gdrn_conv_dgrad_s2(const void* du_hi, const void* du_lo, const vo
     cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
     if (nsplit != 1 && nsplit != 3) return set_error(GDRN_ERR_ARG, "conv_dgrad_s2: nsplit must be 1 or 3");
     if (nsplit == 3 && (du_lo == nullptr || w_lo == nullptr)) return set_error(GDRN_ERR_ARG, "conv_dgrad_s2: lo planes missing");
-    if (!((K == 3 && pad == 1) || (K == 1 && pad == 0))) return set_error(GDRN_ERR_ARG, "conv_dgrad_s2: k3 p1 or k1 p0 only");
+    if (!((K == 3 && pad == 1) || (K == 1 && pad == 0) || (K == 4 && pad == 1) || (K == 2 && pad == 0)))
+        return set_error(GDRN_ERR_ARG, "conv_dgrad_s2: k3 p1, k1 p0, k4 p1 or k2 p0 only (got k%d p%d)", K, pad);
     if (Cy % 64 != 0) return set_error(GDRN_ERR_ARG, "conv_dgrad_s2: Cy=%d must be a multiple of 64", Cy);
     if (ldc % 8 != 0 || ldc < Cx) return set_error(GDRN_ERR_ARG, "conv_dgrad_s2: bad ldc=%d", ldc);
     if (Wo > 128 || 128 % Wo != 0 || (Ho & (Ho - 1)) != 0) return set_error(GDRN_ERR_ARG, "conv_dgrad_s2: unsupported dY size %dx%d", Ho, Wo);
@@ -639,7 +641,7 @@ extern "C" int gdrn_conv_dgrad_s2(const void* du_hi, const void* du_lo, const vo
     const int TN = 128 / (Wo * TH);
     if (Ho % TH != 0) return set_error(GDRN_ERR_ARG, "conv_dgrad_s2: Ho=%d not divisible by tile rows %d", Ho, TH);
     const int num_m_tiles = (N * Ho * Wo + 127) / 128;
-    const int nphase = K == 3 ? 4 : 1;
+    const int nphase = K == 1 ? 1 : 4;
     const int block_n = pick_block_n(Cx_pad, num_m_tiles * nphase);
     if (block_n < 0) return set_error(GDRN_ERR_ARG, "conv_dgrad_s2: Cx_pad=%d must be a multiple of 64", Cx_pad);
 
@@ -678,12 +680,12 @@ extern "C" int gdrn_conv_dgrad_s2(const void* du_hi, const void* du_lo, const vo
     p.act = act & ~kActStatsF64;  // bias / activation (folded eval BatchNorm) and the BatchNorm batch statistics apply to its output
     p.stats = stats;
     p.stats_f64 = (act & kActStatsF64) ? 1 : 0;
-    // phases in order of decreasing tap count (longest tiles first on the persistent CTAs)
+    // phases in order of decreasing tap count (longest tiles first on the persistent CTAs; k = 4 and k = 2 phases are all equal)
     p.nphase = nphase;
     int nt = 0;
     const int order[4][2] = {{1, 1}, {1, 0}, {0, 1}, {0, 0}};
     for (int q = 0; q < nphase; ++q) {
-        const int a = K == 3 ? order[q][0] : 0, b = K == 3 ? order[q][1] : 0;
+        const int a = K == 1 ? 0 : order[q][0], b = K == 1 ? 0 : order[q][1];
         p.ph_a[q] = a;
         p.ph_b[q] = b;
         p.ph_tap0[q] = nt;
@@ -698,7 +700,7 @@ extern "C" int gdrn_conv_dgrad_s2(const void* du_hi, const void* du_lo, const vo
             }
         }
     }
-    p.ph_tap0[nphase] = nt;
+    p.ph_tap0[nphase] = nt;  // <= 16 = sizeof(p.tap_dh)
     p.num_kb = nt * p.cchunks;  // bookkeeping only (per-tile counts come from the phase table)
     for (p.pw_log2 = 0; (1 << p.pw_log2) < Wo; ++p.pw_log2) {}
     for (p.ph_log2 = 0; (1 << p.ph_log2) < Ho; ++p.ph_log2) {}

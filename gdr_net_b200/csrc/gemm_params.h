@@ -32,7 +32,7 @@ struct GemmParams {
     int nphase;
     int ph_tap0[5];
     int ph_a[4], ph_b[4];
-    signed char tap_dh[12], tap_dw[12], tap_w[12];
+    signed char tap_dh[16], tap_dw[16], tap_w[16];  // 16 = the four 2x2-tap phases of k = 4
     int pw_log2, ph_log2;  // log2 of the dY width / height
     // Grouped variant (gemm_fwd_grouped_kernel only): output rows [g * rows_per_group, (g + 1) * rows_per_group) use weight rows
     // [group[g] * w_group_rows, ...) and bias + group[g] * bias_stride; group[g] is clamped to [0, num_w_groups).

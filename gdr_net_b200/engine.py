@@ -233,6 +233,10 @@ class Engine:
         self.mask_loss = MASK_LOSSES[rh.MASK_LOSS_TYPE]
         self.mask_out = 2 if self.mask_loss == MASK_LOSSES["CE"] else 1
         self.n_logits = self.mask_out + 4 + self.num_regions  # per crop: mask | xyz | bg | R regions
+        # head shape (ROT_HEAD.CONV_KERNEL_SIZE, OUT_CONV_KERNEL_SIZE; GDRN.check_head_shape): the deconv's kernel k and padding
+        # (k3 p1 op1, k4 p1, k2 p0: 8x8 -> 16x16 every time) and the output conv's kernel (1 or 3, pad k // 2: 64x64 logits)
+        hf = model.rot_head_net.features
+        self.deconv_k, self.deconv_pad, self.out_k = hf[0].kernel_size[0], hf[0].padding[0], hf[23].kernel_size[0]
         # class-aware head (ROT_HEAD.*_CLASS_AWARE): the output conv holds per-class rows (class_rows) and every crop's logits come
         # from its class's rows, selected per 128-row tile by the grouped GEMMs -- the logit row layout stays the one above
         aware = (bool(rh.ROT_CLASS_AWARE), bool(rh.MASK_CLASS_AWARE), bool(rh.REGION_CLASS_AWARE))
@@ -338,7 +342,7 @@ class Engine:
         self.cls_npad, self.cls_rows = npad, n_rows
         self.cls_idx = torch.from_numpy(idx).to(self.dev)
         self.cls_slot = torch.from_numpy(slot).to(self.dev)
-        self.w_cls = torch.zeros(C_ * npad, 256, device=self.dev)
+        self.w_cls = torch.zeros(C_ * npad, 256 * self.out_k * self.out_k, device=self.dev)
         self.b_cls = torch.zeros(C_ * npad, device=self.dev)
 
     def _classes(self, roi_classes, B: int) -> torch.Tensor:
@@ -387,7 +391,8 @@ class Engine:
         if self.class_aware:  # the class-major tables the pack jobs of the output conv read
             w23 = self.model.rot_head_net.features[23]
             n = self.num_classes * self.cls_npad
-            C.gdrn_class_gather(w23.weight.data_ptr(), self.cls_idx.data_ptr(), self.w_cls.data_ptr(), n, 256, self.cls_rows, _stream())
+            C.gdrn_class_gather(w23.weight.data_ptr(), self.cls_idx.data_ptr(), self.w_cls.data_ptr(), n, self.w_cls.shape[1],
+                                self.cls_rows, _stream())
             C.gdrn_class_gather(w23.bias.data_ptr(), self.cls_idx.data_ptr(), self.b_cls.data_ptr(), n, 1, self.cls_rows, _stream())
         C.gdrn_pack_weight_batched(tab["jobs"].data_ptr(), tab["njobs"], tab["blocks"], _stream())
 
@@ -490,11 +495,12 @@ class Engine:
         def cbr(xin, ck, bk, conv, relu=True, res=None):
             gn = self._gn_mods.get(bk)
             if gn is not None:  # GroupNorm head: the unfolded conv, then GroupNorm + ReLU
-                u = (ops.conv_dgrad_s2(xin, self.wf[ck], conv.out_channels, 3, 1) if ck == "deconv"
+                u = (ops.conv_dgrad_s2(xin, self.wf[ck], conv.out_channels, self.deconv_k, self.deconv_pad) if ck == "deconv"
                      else ops.conv_fwd(xin, self.wf[ck], conv.out_channels, 3, 3, 1, 1))
                 return ops.head_gn_relu_fwd(u, gn.weight, gn.bias, gn.num_groups, gn.eps)[0]
             if ck == "deconv":
-                return ops.conv_dgrad_s2(xin, wfe[ck], conv.out_channels, 3, 1, bias=shift[bk], act=2 if relu else 0)
+                return ops.conv_dgrad_s2(xin, wfe[ck], conv.out_channels, self.deconv_k, self.deconv_pad, bias=shift[bk],
+                                         act=2 if relu else 0)
             k, stride, pad = conv.kernel_size[0], conv.stride[0], conv.padding[0]
             return ops.conv_fwd(xin, wfe[ck], conv.out_channels, k, k, stride, pad, bias=shift[bk], act=2 if relu else 0, res=res)
 
@@ -539,7 +545,7 @@ class Engine:
         return {k: (v.clone() if isinstance(v, torch.Tensor) else v) for k, v in res.items()}
 
     def _head_pnp(self, head_in: PT, aux: dict, pnp_saved: Optional[list] = None, train: bool = False):
-        """1x1 output conv -> glue -> Patch-PnP (GDRN.py:156-181, conv_pnp_net.py:111-157).  Returns the fp32 logits
+        """output conv (1x1 or 3x3) -> glue -> Patch-PnP (GDRN.py:156-181, conv_pnp_net.py:111-157).  Returns the fp32 logits
         [B*4096, 72] (n_logits valid), the Patch-PnP input planes [B, 64, 64, pnp_ld], pred [B, 16] (cols 0..5 rot6d, 6..8 centroid dx, dy and z), the inputs
         of the three FC layers and the DropBlock (keep, scale) of a train-mode forward with drop_prob > 0, else None; pnp_saved
         receives the Patch-PnP conv activations (pnp_net_forward)."""
@@ -547,9 +553,10 @@ class Engine:
         logits = torch.empty(B * 4096, 72, device=dev)
         if self.class_aware:  # crop b (4096 rows) reads the weight / bias block of class roi_classes[b]
             ops.conv_fwd_grouped(head_in, self.wf["rot_head_net.features.23"], self.n_logits, self.cls_npad, aux["roi_classes"], 4096,
-                                 out_f32=logits, bias=self.b_cls, bias_stride=self.cls_npad, ldc=72)
+                                 out_f32=logits, bias=self.b_cls, bias_stride=self.cls_npad, ldc=72, k=self.out_k)
         else:
-            ops.conv_fwd(head_in, self.wf["rot_head_net.features.23"], self.n_logits, 1, 1, 1, 0, out_f32=logits,
+            k = self.out_k
+            ops.conv_fwd(head_in, self.wf["rot_head_net.features.23"], self.n_logits, k, k, 1, k // 2, out_f32=logits,
                          bias=m.rot_head_net.features[23].bias, ldc=72, want_planes=False)
         pnp_in = PT((B, 64, 64, self.pnp_ld), self.planes, device=dev)
         glue = (logits.data_ptr(), ops.ptr(aux.get("roi_coord_2d")), aux["roi_extents"].data_ptr(), pnp_in.hi_ptr, pnp_in.lo_ptr, B, 4096,
@@ -566,7 +573,7 @@ class Engine:
         return logits, pnp_in, pred, fc_in, db
 
     def _tail_inference(self, head_in: PT, aux: dict, want_maps: bool, train: bool) -> dict:
-        """1x1 output conv -> glue -> Patch-PnP -> test-time pose decode (shared by the folded and the plain eval forward);
+        """output conv -> glue -> Patch-PnP -> test-time pose decode (shared by the folded and the plain eval forward);
         train: DropBlock applies (a train-mode forward without losses)."""
         B = head_in.shape[0]
         logits, _, pred, _, _ = self._head_pnp(head_in, aux, train=train)
@@ -625,12 +632,13 @@ class Engine:
         wf["stem"] = ops.pack_stem(m.backbone.conv1.weight, pl, out=wf.get("stem"))
 
     def _class_head_pack_calls(self, need_dgrad: bool):
-        """Class-aware output conv: forward operand [C * cls_npad][256] and dgrad operand [C][256][128] from the class-major table."""
-        key, C_, npad = "rot_head_net.features.23", self.num_classes, self.cls_npad
-        src = self.w_cls.view(C_ * npad, 256, 1, 1)
+        """Class-aware output conv: forward operand [C * cls_npad][k * k * 256] and dgrad operand [C][256][k * k * 128] from the
+        class-major table."""
+        key, C_, npad, k = "rot_head_net.features.23", self.num_classes, self.cls_npad, self.out_k
+        src = self.w_cls.view(C_ * npad, 256, k, k)
         self.wf[key] = ops.pack_conv_fwd(src, self.planes, out=self.wf.get(key))
         if need_dgrad:
-            wd = self.wd.get(key) or PT((C_ * 256, 128), self.bplanes, device=self.dev)
+            wd = self.wd.get(key) or PT((C_ * 256, k * k * 128), self.bplanes, device=self.dev)
             self.wd[key] = wd
             for c in range(C_):
                 ops.pack_conv_dgrad(src[c * npad:(c + 1) * npad], self.bplanes, out=_PlaneRows(wd, c * 256), ipad=128)
@@ -672,7 +680,7 @@ class Engine:
         stats = self.bn[bkey].stats64 if (gn is None and train_bn and not self.deterministic) else None
         k, stride, pad = conv.kernel_size[0], conv.stride[0], conv.padding[0]
         if ckey == "deconv":
-            u = ops.conv_dgrad_s2(x, self.wf["deconv"], conv.out_channels, 3, 1, stats=stats)
+            u = ops.conv_dgrad_s2(x, self.wf["deconv"], conv.out_channels, self.deconv_k, self.deconv_pad, stats=stats)
         else:
             u = ops.conv_fwd(x, self.wf[ckey], conv.out_channels, k, k, stride, pad, stats=stats)
         if gn is not None:
@@ -1010,9 +1018,16 @@ class Engine:
             C.gdrn_head_bwd_ex(*hb, _stream())
         hf = m.rot_head_net.features
         head_in = h(S["head_in"])
-        n_out = self.n_logits  # rows of the 1x1 output conv
+        n_out = self.n_logits  # rows of the output conv
         if self.class_aware:
             g = self._class_head_bwd(dlog, head_in, aux["roi_classes"], B)
+        elif self.out_k == 3:  # the 3x3 output conv over dlog viewed as [B, 64, 64, 128]: conv wgrad and dgrad, bias as below
+            dlog4 = dlog.view(B, 64, 64, 128)
+            self._wgrad_conv(dlog4, head_in, hf[23], "rot_head_net.features.23.weight")
+            tmp128 = torch.empty(128, device=dev)
+            C.gdrn_colsum(dlog.hi_ptr, dlog.lo_ptr, tmp128.data_ptr(), B * 4096, 128, _stream())
+            self.grads["rot_head_net.features.23.bias"].copy_(tmp128[:n_out])
+            g = self._dgrad_conv(dlog4, hf[23], "rot_head_net.features.23")
         else:
             def head_out_wgrad():
                 buf, ks, kss = ops.gemm_wgrad(dlog, head_in.view(B * 4096, 256), self.ws)
@@ -1034,17 +1049,19 @@ class Engine:
                 g = ops.upsample2x_bwd(g)
         D = S["deconv"]
         du = self._head_norm_bwd("rot_head_net.features.1", g, h(D["u"]), D)
+        k, pad = self.deconv_k, self.deconv_pad
+
         def deconv_wgrad(du=du):
-            # d wt[ci][co][r][s] = sum_q x[ci][q] * du[co][2q + (r, s) - 1]: the weight gradient of the stride-2 conv du -> x
-            # with x in the role of dY; its [O = 512][I = 256][3][3] layout IS the ConvTranspose2d IOHW layout (no flip)
-            buf, ks, kss = ops.conv_wgrad(h(D["z"]), du, self.ws, 512, 3, 3, 2, 1)
-            ops.unpack_wgrad(buf, self.grads["rot_head_net.features.0.weight"], 512, 256, 3, 3, 256, ks, kss, 256 * 9, 9, 3, 1)
+            # d wt[ci][co][r][s] = sum_q x[ci][q] * du[co][2q + (r, s) - pad]: the weight gradient of the stride-2 conv du -> x
+            # with x in the role of dY; its [O = 512][I = 256][k][k] layout IS the ConvTranspose2d IOHW layout (no flip)
+            buf, ks, kss = ops.conv_wgrad(h(D["z"]), du, self.ws, 512, k, k, 2, pad)
+            ops.unpack_wgrad(buf, self.grads["rot_head_net.features.0.weight"], 512, 256, k, k, 256, ks, kss, 256 * k * k, k * k, k, 1)
 
         self._on_side(deconv_wgrad, keep=(du,))
         if not self.live_bb:  # frozen backbone: the head's gradients end the step
             self._segment_done("rot_head_net")
             return self._backward_done()
-        g = ops.conv_fwd(du, self.wd["deconv"], 512, 3, 3, 2, 1)  # [B,8,8,512]
+        g = ops.conv_fwd(du, self.wd["deconv"], 512, k, k, 2, pad)  # [B,8,8,512]
         self._segment_done("rot_head_net")
 
         # ---- backbone (torchvision BasicBlock backward)
@@ -1089,19 +1106,31 @@ class Engine:
     def _class_head_bwd(self, dlog: PT, head_in: PT, classes: torch.Tensor, B: int) -> PT:
         """Backward of the class-aware output conv: the grouped dgrad on the main stream; on the side stream the per-crop weight
         partials (the wgrad GEMM split at crop boundaries, ksplit = B) and per-crop bias partials, reduced in crop order into the
-        reference layout (rows of classes absent from the batch get exactly 0)."""
+        reference layout (rows of classes absent from the batch get exactly 0).  A 3x3 output conv runs the conv wgrad, split the
+        same way (4096 pixels = 64 k-blocks per crop), and the grouped 3x3 dgrad; its partials are tap-major ([row][tap][ci]), so
+        they are reduced into a scratch table that is then unpacked into the OIHW gradient."""
+        k, key = self.out_k, "rot_head_net.features.23"
+
         def work():
-            buf, ks, kss = ops.gemm_wgrad(dlog, head_in.view(B * 4096, 256), self.ws, ksplit=B)
+            if k == 1:
+                buf, ks, kss = ops.gemm_wgrad(dlog, head_in.view(B * 4096, 256), self.ws, ksplit=B)
+            else:
+                buf, ks, kss = ops.conv_wgrad(dlog.view(B, 64, 64, 128), head_in, self.ws, self.n_logits, k, k, 1, k // 2, ksplit=B)
             assert ks == B, (ks, B)  # 4096 rows = 64 k-blocks per split: split b is crop b
             bias_part = torch.empty(B, 128, device=self.dev)
             C.gdrn_crop_colsum(dlog.hi_ptr, dlog.lo_ptr, bias_part.data_ptr(), B, 4096, 128, _stream())
-            C.gdrn_class_wgrad_reduce(buf.data_ptr(), kss, 256, bias_part.data_ptr(), 128, classes.data_ptr(), B,
-                                      self.cls_slot.data_ptr(), self.num_classes, self.cls_rows, self.n_logits, 256,
-                                      self.grads["rot_head_net.features.23.weight"].data_ptr(),
-                                      self.grads["rot_head_net.features.23.bias"].data_ptr(), _stream())
+            K = k * k * 256
+            gw = self.grads[key + ".weight"] if k == 1 else torch.empty(self.cls_rows, K, device=self.dev)
+            C.gdrn_class_wgrad_reduce(buf.data_ptr(), kss, K, bias_part.data_ptr(), 128, classes.data_ptr(), B,
+                                      self.cls_slot.data_ptr(), self.num_classes, self.cls_rows, self.n_logits, K,
+                                      gw.data_ptr(), self.grads[key + ".bias"].data_ptr(), _stream())
+            if k != 1:
+                ops.unpack_wgrad(gw, self.grads[key + ".weight"], self.cls_rows, 256, k, k, 256, 1, 0, K, k * k, k, 1)
 
         self._on_side(work, keep=(dlog, classes))
-        return ops.gemm_fwd_grouped(dlog, self.wd["rot_head_net.features.23"], 256, classes, 4096).view(B, 64, 64, 256)
+        if k == 1:
+            return ops.gemm_fwd_grouped(dlog, self.wd[key], 256, classes, 4096).view(B, 64, 64, 256)
+        return ops.conv_fwd_grouped(dlog.view(B, 64, 64, 128), self.wd[key], 256, 256, classes, 4096, k=k)
 
     def materialize_aliased_grads(self):
         """A p.grad that still aliases flat_grad (adopted by autograd in an earlier step and not reset by zero_grad) would be

@@ -233,8 +233,9 @@ def conv_fwd(x: PT, wp: PT, Cout: int, KH: int, KW: int, stride: int, pad: int, 
 
 
 def conv_dgrad_s2(du: PT, wd: PT, Cx: int, K: int, pad: int, *, out: PT | None = None, bias=None, stats=None, act: int = 0) -> PT:
-    """dX of a stride-2 conv (k3 p1 / k1 p0) from the UN-dilated dY, decomposed by output parity (gdrn_conv_dgrad_s2);
-    wd = pack_conv_dgrad(weight).  Replaces zero_insert + stride-1 conv (4x the MACs, plus the dilated tensor in HBM)."""
+    """dX of a stride-2 conv (k3 p1 / k1 p0 / k4 p1 / k2 p0) from the UN-dilated dY, decomposed by output parity
+    (gdrn_conv_dgrad_s2); wd = pack_conv_dgrad(weight).  Replaces zero_insert + stride-1 conv (4x the MACs, plus the dilated
+    tensor in HBM).  With wd = pack_conv_dgrad of a ConvTranspose2d weight it is that layer's forward."""
     N, Ho, Wo, Cy = du.shape
     ldc = _round_up(Cx, 64)
     if out is None:
@@ -256,15 +257,19 @@ def gemm_fwd(a: PT, wp: PT, N: int, *, out: PT | None = None, out_f32: torch.Ten
     return out
 
 
-def conv_fwd_grouped(x: PT, wp: PT, Cout: int, Cout_pad: int, group: torch.Tensor, rows_per_group: int, *, out_f32: torch.Tensor,
-                     bias=None, bias_stride: int = 0, ldc: int | None = None):
-    """1x1 / k x k stride-1 conv whose output rows [g * rows_per_group, ...) use weight block group[g] of wp ([G * Cout_pad][K]) and
-    bias[group[g] * bias_stride:]; group: int32 device tensor.  fp32 output only (the class-aware output conv's logits)."""
+def conv_fwd_grouped(x: PT, wp: PT, Cout: int, Cout_pad: int, group: torch.Tensor, rows_per_group: int, *,
+                     out_f32: torch.Tensor | None = None, bias=None, bias_stride: int = 0, ldc: int | None = None, k: int = 1):
+    """k x k (k = 1 or 3, pad k // 2) stride-1 conv whose output rows [g * rows_per_group, ...) use weight block group[g] of wp
+    ([G * Cout_pad][K]) and bias[group[g] * bias_stride:]; group: int32 device tensor.  Writes out_f32 (the class-aware output conv's
+    logits) if given, else returns 16-bit planes [N, H, W, ldc] like x's (its 3x3 data gradient)."""
     N, H, W, Cin = x.shape
     G = wp.shape[0] // Cout_pad
-    C.gdrn_conv_fwd_grouped(x.hi_ptr, x.lo_ptr, wp.hi_ptr, wp.lo_ptr, None, None, out_f32.data_ptr(), ptr(bias), N, H, W, Cin, Cout,
-                            Cout_pad, 1, 1, 1, 0, ldc or _round_up(Cout, 64), 0, x.nsplit, group.data_ptr(), rows_per_group, G,
-                            bias_stride, _stream())
+    ldc = ldc or _round_up(Cout, 64)
+    out = None if out_f32 is not None else PT((N, H, W, ldc), x.planes, device=x.buf.device, zero=(ldc != Cout))
+    C.gdrn_conv_fwd_grouped(x.hi_ptr, x.lo_ptr, wp.hi_ptr, wp.lo_ptr, out.hi_ptr if out is not None else None,
+                            out.lo_ptr if out is not None else None, ptr(out_f32), ptr(bias), N, H, W, Cin, Cout, Cout_pad, k, k, 1,
+                            k // 2, ldc, 0, x.nsplit, group.data_ptr(), rows_per_group, G, bias_stride, _stream())
+    return out
 
 
 def gemm_fwd_grouped(a: PT, wp: PT, N: int, group: torch.Tensor, rows_per_group: int) -> PT:

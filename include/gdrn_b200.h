@@ -51,11 +51,12 @@ int gdrn_conv_fwd(const void* x_hi, const void* x_lo, const void* w_hi, const vo
                   int Cin, int Cout, int Cout_pad, int KH, int KW, int stride, int pad, int ldc, int act, int nsplit,
                   void* stream);
 
-/* Data gradient of a stride-2 conv (k3 p1 / k1 p0) by output-parity phases over the un-dilated dY: replaces the reference's
- * cuDNN conv-backward-data for the stride-2 layers (resnet_backbone.py layerN.0.conv1 / downsample, conv_pnp_net.py:76-80).
- * du [N][Ho][Wo][Cy], w = dgrad-packed weights (flipped taps), dx [N][2Ho][2Wo][ldc]; k1: dx must be pre-zeroed.
- * The same arithmetic is the FORWARD of nn.ConvTranspose2d(k3, s2, p1, output_padding 1) (cdpn_rot_head_region.py:82-91; its IOHW
- * weight is the OIHW weight of the transposed conv): bias / act / stats (optional) then apply to the output like gdrn_conv_fwd. */
+/* Data gradient of a stride-2 conv (k3 p1 / k1 p0 / k4 p1 / k2 p0; any other pair is GDRN_ERR_ARG) by output-parity phases over
+ * the un-dilated dY: replaces the reference's cuDNN conv-backward-data for the stride-2 layers (resnet_backbone.py layerN.0.conv1 /
+ * downsample, conv_pnp_net.py:76-80).  du [N][Ho][Wo][Cy], w = dgrad-packed weights (flipped taps), dx [N][2Ho][2Wo][ldc];
+ * k1: dx must be pre-zeroed.  The same arithmetic is the FORWARD of the geometry head's nn.ConvTranspose2d(k, s2, p, op) --
+ * k3 p1 op1, k4 p1 op0 or k2 p0 op0 (ROT_HEAD.CONV_KERNEL_SIZE, cdpn_rot_head_region.py:33-41, 81-91; its IOHW weight is the OIHW
+ * weight of the transposed conv): bias / act / stats (optional) then apply to the output like gdrn_conv_fwd, in every phase. */
 int gdrn_conv_dgrad_s2(const void* du_hi, const void* du_lo, const void* w_hi, const void* w_lo, void* dx_hi, void* dx_lo,
                        const float* bias, float* stats, int N, int Ho, int Wo, int Cy, int Cx, int Cx_pad, int K, int pad, int ldc,
                        int act, int nsplit, void* stream);
@@ -67,6 +68,7 @@ int gdrn_gemm_fwd(const void* a_hi, const void* a_lo, const void* w_hi, const vo
                   int nsplit, void* stream);
 
 /* ---- class-aware output conv (ROT_HEAD.*_CLASS_AWARE; GDRN.py:134-151, cdpn_rot_head_region.py:114-135): grouped GEMMs.
+ * gdrn_conv_fwd_grouped takes a 1x1 or a 3x3 stride-1 conv (OUT_CONV_KERNEL_SIZE; TMA zero fill supplies every crop's border).
  * w holds num_groups blocks of Cout_pad (N_pad) rows, [num_groups * Cout_pad][K]; bias num_groups blocks of bias_stride floats.
  * Output rows [g * rows_per_group, (g + 1) * rows_per_group) use block group[g] (device int array of M / rows_per_group entries,
  * clamped to [0, num_groups)); rows_per_group % 128 == 0, so no 128-row tile straddles two groups.  No residual, no statistics. */
