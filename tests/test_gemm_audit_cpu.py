@@ -143,6 +143,27 @@ def test_excess_measure():
     assert GA.excess(torch.tensor([1.0, float("nan"), 0.0, 4.0]), ref, absref) == (math.inf, 1)  # an unwritten element
 
 
+def test_stats_err_takes_off_the_storage_rounding_only():
+    """Sums of fp32 values against the fp16-stored values: the rounding noise of the store is not charged, a row missing
+    from one channel's sums still is."""
+    g = torch.Generator().manual_seed(3)
+    f = torch.randn(16384, 256, generator=g) * torch.linspace(0.01, 10.0, 256)  # a pre-BatchNorm output, channel scales apart
+    f[:, 7] = torch.relu(f[:, 7]) ** 3  # a heavy-tailed channel
+    stats = torch.stack([f.double().sum(0), (f.double() ** 2).sum(0)]).float()  # what the epilogue sums (fp32 here)
+    y = f.half().double()  # what the store kept
+    u = torch.finfo(torch.float16).eps / 2
+    assert GA.stats_err(stats, y) > GA.STATS_BOUND  # the rounding alone exceeds the bound when it is charged
+    assert GA.stats_err(stats, y, u) < GA.STATS_BOUND / 4
+    # one row of median magnitude of a Gaussian channel; of the heavy-tailed channel one of its top 3 %, whose sums of squares
+    # are dominated, and their rounding noise set, by a few rows
+    for col, rank in ((100, 8192), (7, 16000)):
+        row = int(f[:, col].abs().argsort()[rank])
+        bad = stats.clone()
+        bad[0, col] -= f[row, col]
+        bad[1, col] -= f[row, col] ** 2
+        assert GA.stats_err(bad, y, u) > GA.STATS_BOUND, col
+
+
 def test_tile_width_choice():
     assert GA.pick_block_n(128, 64, 132) == 64     # 2 x 64 x 64 pixels, 128 channels: 64 tiles, below half a wave
     assert GA.pick_block_n(256, 2048, 132) == 128  # the 64 x 64 x 256 head layers at B = 64
@@ -162,9 +183,45 @@ def test_persistent_grid():
     g = GA.fwd_grid(64 * 32 * 32, 64, 4, 132)  # layer2.0.conv1's stride-2 dgrad at B = 64: 4 phases x 512 tiles
     assert (g["block_n"], g["groups"], g["ctas"], g["max_per_cta"], g["remainder"]) == (64, 2048, 132, 16, 68)
     t = GA.tile_of(g, 130, 5, phase=2)  # group 2 * 512 + 1 = 1025 -> CTA 1025 % 132 = 101, its 8th tile
-    assert t == dict(m_tile=1, n_tile=0, phase=2, cta=101, tiles_before=7)
+    assert t == dict(m_tile=1, n_tile=0, phase=2, box=0, warpgroup=0, half=0, cta=101, tiles_before=7)
     g = GA.fwd_grid(512 * 128, 128, 0, 132)
-    assert GA.tile_of(g, 128 * 200 + 3, 100) == dict(m_tile=200, n_tile=0, phase=0, cta=68, tiles_before=1)
+    assert GA.tile_of(g, 128 * 200 + 3, 100) == dict(m_tile=200, n_tile=0, phase=0, box=0, warpgroup=0, half=0, cta=68, tiles_before=1)
+    assert GA.tile_of(g, 128 * 3 + 70, 0) == dict(m_tile=3, n_tile=0, phase=0, box=0, warpgroup=1, half=0, cta=3, tiles_before=0)
+
+
+def test_tile_height_choice():
+    """pick_block_m at 132 SMs: 256-row tiles need nsplit 1, the 128-wide tile, a plain epilogue and ceil(M / 256) * n-tiles
+    >= 99."""
+    l2c1 = 64 * 32 * 32  # layer2.0.conv1 at B = 64 (3x3 s2, 64 -> 128): 512 128-row tiles, 256 tall ones
+    assert GA.pick_block_m(l2c1, 128, 1, True, 132) == 256
+    assert GA.pick_block_m(l2c1, 128, 1, False, 132) == 128  # the same launch with epilogue statistics (or a residual, ...)
+    assert GA.pick_block_m(l2c1, 128, 3, True, 132) == 128   # 3-pass
+    assert GA.pick_block_m(64 * 8 * 8, 512, 1, True, 132) == 128  # layer4: 32 x 4 128-wide tiles, only 16 x 4 = 64 tall ones
+    assert GA.pick_block_m(64 * 16 * 16, 256, 1, True, 132) == 256  # layer3.0.conv1: 64 x 2 = 128 tall tiles
+    assert GA.pick_block_m(99 * 256, 128, 1, True, 132) == 256 and GA.pick_block_m(98 * 256, 128, 1, True, 132) == 128
+    assert GA.pick_block_m(98 * 256 + 1, 128, 1, True, 132) == 256  # a partial last tall tile counts
+    assert GA.pick_block_m(64 * 64 * 64, 64, 1, True, 132) == 128  # layer1: 64 wide
+    g = GA.fwd_grid(l2c1, 128, 0, 132, block_m=256)
+    assert (g["block_n"], g["num_m"], g["groups"], g["ctas"], g["max_per_cta"], g["remainder"]) == (128, 256, 256, 132, 2, 124)
+    g = GA.fwd_grid(l2c1, 128, 0, 132)
+    assert (g["block_m"], g["num_m"], g["groups"], g["max_per_cta"], g["remainder"]) == (128, 512, 512, 4, 116)
+
+
+def test_tall_tiles_with_two_images_per_box():
+    """Patch-PnP features.6 at B = 512 (3x3 s2, 16^2 -> 8^2, 128 -> 128): one 128-row A box holds TN = 2 images of 8 x 8 rows, a
+    tall tile 4 images; 128 tall tiles, one per CTA."""
+    M = 512 * 8 * 8
+    assert GA.a_box_images(8, 8) == 2 and GA.a_box_images(16, 16) == 1 and GA.a_box_images(32, 32) == 1 and GA.a_box_images(4, 4) == 8
+    assert GA.pick_block_m(M, 128, 1, True, 132) == 256
+    g = GA.fwd_grid(M, 128, 0, 132, block_m=256)
+    assert (g["block_n"], g["num_m"], g["groups"], g["ctas"], g["max_per_cta"], g["remainder"]) == (128, 128, 128, 128, 1, 0)
+    # image 22 = row 1408 + 3 * 8 + 1: tall tile 5 (images 20..23), box 1 (images 22, 23) of warpgroup 1, its first 64-row half
+    assert GA.tile_of(g, 22 * 64 + 3 * 8 + 1, 7) == dict(m_tile=5, n_tile=0, phase=0, box=1, warpgroup=1, half=0, cta=5, tiles_before=0)
+    # image 21, last row: box 0, second half of warpgroup 0
+    assert GA.tile_of(g, 22 * 64 - 1, 7) == dict(m_tile=5, n_tile=0, phase=0, box=0, warpgroup=0, half=1, cta=5, tiles_before=0)
+    # layer2.0.conv1's tall grid: row 200 of tall tile 200 = box 1, half 1; group 200 is CTA 68's second tile
+    g = GA.fwd_grid(64 * 32 * 32, 128, 0, 132, block_m=256)
+    assert GA.tile_of(g, 256 * 200 + 200, 127) == dict(m_tile=200, n_tile=0, phase=0, box=1, warpgroup=1, half=1, cta=68, tiles_before=1)
 
 
 def test_wgrad_tiles_and_ksplit():

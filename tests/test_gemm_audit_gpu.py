@@ -4,7 +4,10 @@ The engine runs eagerly on one stream on the benchmark's workload (seeded weight
 each launch of gemm_fwd_kernel / gemm_wgrad_kernel is compared element by element with a float64 reference built from that
 launch's own operands.  At B = 64 almost every launch gives a persistent CTA 2..60 tiles, on the 128-wide tiles that do
 most of the work: the shapes the synthetic op tests (tests/test_ops_gpu.py, tests/test_engine_ops_gpu.py) do not reach.
-test_coverage_b64 asserts that the audit reached what it was written for."""
+The single-pass "half" mode runs the same B = 64 step and the stand-alone Patch-PnP at the benchmark's B = 512: its
+large plain-epilogue forwards (the stride-2 convs among them) are the launches of the 256-row tile, and its epilogue
+statistics and folded epilogues are the nsplit-1 variants of the mixed mode's.  test_coverage_b64 asserts that the audit
+reached what it was written for."""
 import time
 
 import pytest
@@ -58,19 +61,46 @@ def _label(eng):
     return label
 
 
+def _patch_pnp(precision, B, nIn=69):
+    """The stand-alone Patch-PnP of the benchmark (seeded weights and maps), eagerly: () -> runs one forward, and its label."""
+    from gdr_net_b200 import ops, synth
+    from gdr_net_b200.GDRN import ConvPnPNet
+    from gdr_net_b200.patch_pnp import PatchPnP
+
+    net = ConvPnPNet(nIn=nIn).cuda()
+    sd = synth.seeded_state_dict({"pnp_net." + k: v for k, v in net.state_dict().items()}, seed=11)
+    net.load_state_dict({k[len("pnp_net."):]: v for k, v in sd.items()})
+    net.eval()
+    g = synth._gen(7, "pnp_bench")
+    coor = torch.rand(B, nIn - 64, 64, 64, generator=g).cuda()
+    region = torch.softmax(2.0 * torch.randn(B, 64, 64, 64, generator=g), dim=1).cuda()
+    ext = (0.05 + 0.25 * torch.rand(B, 3, generator=g)).cuda()
+    runner = PatchPnP(net, precision)
+    runner.use_cuda_graphs = False  # eager: each wrapper reads its launch's result right after it
+    runner(coor, region, ext)  # packs the weights, so that the label can name them
+    torch.cuda.synchronize()
+
+    def label(wp):  # (wf also holds the fp32 w_rt / b_rt the fc_rt operand is packed from)
+        return next((f"wf[{k}]" for k, t in runner.wf.items() if isinstance(t, ops.PT) and t.buf.data_ptr() == wp.buf.data_ptr()), "?")
+
+    return (lambda: runner(coor, region, ext)), label
+
+
 RUNS = {}  # name -> (records, launches seen at the C ABI, seconds) or the exception of a failed audit (never re-run)
 
 
 def _run(name, precision="mixed", B=64, mode="train"):
     if name not in RUNS:
-        model, eng, x, aux = _engine(precision, B)
-        if mode == "eval":  # move the running statistics off their initial (0, 1), so the folded row scales differ per channel
-            eng.forward(x[:4].contiguous(), {k: (v[:4].contiguous() if isinstance(v, torch.Tensor) else v) for k, v in aux.items()},
-                        train_bn=True, do_loss=False)
-        torch.cuda.synchronize()
-        t0 = time.time()
-        try:
-            with GA.Audit(label=_label(eng)) as au:
+        if mode == "patch_pnp":
+            step, label = _patch_pnp(precision, B)
+        else:
+            model, eng, x, aux = _engine(precision, B)
+            if mode == "eval":  # move the running statistics off their initial (0, 1), so the folded row scales differ per channel
+                eng.forward(x[:4].contiguous(), {k: (v[:4].contiguous() if isinstance(v, torch.Tensor) else v) for k, v in aux.items()},
+                            train_bn=True, do_loss=False)
+            label = _label(eng)
+
+            def step():
                 if mode == "train":
                     eng.forward(x, aux, train_bn=True, do_loss=True)
                     eng.backward(torch.ones(8, device="cuda"))
@@ -80,12 +110,17 @@ def _run(name, precision="mixed", B=64, mode="train"):
                 else:
                     model.eval()
                     eng.forward_eval_folded(x, aux)
+        torch.cuda.synchronize()
+        t0 = time.time()
+        try:
+            with GA.Audit(label=label) as au:
+                step()
                 torch.cuda.synchronize()
             RUNS[name] = (au.records, au.c_launches, time.time() - t0)
             print(f"{name}: {au.n_audited()} launches audited in {RUNS[name][2]:.1f} s")
         except Exception as e:  # noqa: BLE001 (kept, so that the coverage test reports it instead of repeating the launch)
             RUNS[name] = e
-        del model, eng, x, aux
+        del step, label
         torch.cuda.empty_cache()
     if isinstance(RUNS[name], Exception):
         raise RUNS[name]
@@ -96,7 +131,9 @@ def _run(name, precision="mixed", B=64, mode="train"):
 
 
 B64 = dict(mixed_train=dict(), fp32x3_train=dict(precision="fp32x3"), mixed_atomic_stats=dict(mode="atomic_stats"),
-           mixed_eval_folded=dict(mode="eval"))
+           mixed_eval_folded=dict(mode="eval"), half_train=dict(precision="half"),
+           half_atomic_stats=dict(precision="half", mode="atomic_stats"), half_eval_folded=dict(precision="half", mode="eval"))
+PNP512 = dict(precision="half", B=512, mode="patch_pnp")  # the benchmark's stand-alone Patch-PnP (nIn = 69)
 
 
 @pytest.mark.parametrize("name", list(B64))
@@ -105,13 +142,22 @@ def test_audit_b64(name):
     <256,1> <192,1> <128,1> <64,1>, the fp32 logits with bias and ldc 72, the FC stack, the stem GEMM.  fp32x3 train: 3-pass
     dgrad and weight gradients <128,3> <64,3>.  atomic statistics: the BatchNorm sums of the epilogue over many tiles per
     CTA, incl. the deconvolution forward (4 phases) and the stem.  folded eval: bias + residual + ReLU on 128-wide tiles over
-    row-scaled weights."""
+    row-scaled weights.  half: the same steps single-pass; the large plain-epilogue forwards on 256-row tiles <128,1>, the
+    epilogue statistics and the folded bias / residual epilogues at nsplit 1."""
     records = _run(name, **B64[name])
     ops_seen = {r["op"] for r in records}
     if name.endswith("train"):
         assert ops_seen == set(GA.Audit.OPS), ops_seen
     else:
         assert {"conv_fwd", "gemm_fwd", "conv_dgrad_s2"} <= ops_seen, ops_seen
+
+
+def test_audit_patch_pnp_b512():
+    """Half Patch-PnP at B = 512: the three 3x3 s2 convs on 256-row tiles (64^2 -> 32^2 over the 69 -> 128 padded input,
+    32^2 -> 16^2, and 16^2 -> 8^2 with two images per 128-row A box), then fc1 / fc2 / fc_rt."""
+    records = _run("half_patch_pnp_b512", **PNP512)
+    convs = [r for r in records if r["op"] == "conv_fwd"]
+    assert len(convs) == 3 and all(r["stride"] == 2 and r["KH"] == 3 for r in convs), [r["name"] for r in convs]
 
 
 @pytest.mark.parametrize("B", [3, 20])
@@ -130,10 +176,10 @@ def test_audit_small_batches(B):
 
 def test_coverage_b64():
     """What the B = 64 audits must have reached; computed from the shapes, the variant's width and the SM count."""
-    fwd, wg = [], []
-    for name, kw in B64.items():
+    fwd, wg, runs = [], [], dict(B64, half_patch_pnp_b512=PNP512)
+    for name, kw in runs.items():
         recs = _run(name, **kw)
-        fwd += [r for r in recs if r["op"] in ("conv_fwd", "gemm_fwd", "conv_dgrad_s2")]
+        fwd += [dict(r, run=name) for r in recs if r["op"] in ("conv_fwd", "gemm_fwd", "conv_dgrad_s2")]
         wg += [r for r in recs if r["op"] in ("conv_wgrad", "gemm_wgrad")]
     assert {r["variant"] for r in fwd} == {1283, 643, 1281, 641}
     for v in (1283, 643, 1281, 641):
@@ -144,7 +190,18 @@ def test_coverage_b64():
     assert any(r["stats"] and r["nphase"] == 4 for r in fwd), "the deconvolution forward with epilogue statistics"
     assert {(r["width"], r["nsplit"]) for r in wg} == {(256, 1), (192, 1), (128, 1), (64, 1), (128, 3), (64, 3)}
     assert any(r["ksplit"] > 1 for r in wg)
-    secs = {n: round(RUNS[n][2], 1) for n in B64}
+    # the 256-row tile (at 132 SMs: ceil(M / 256) * n-tiles >= 99).  Mixed reaches it only with the stride-1 dgrads; the half
+    # forward adds layer2.0.conv1 (3x3 s2, 256 tall tiles on 132 CTAs), the layer2.0 / layer3.0 1x1 s2 downsamples and
+    # Patch-PnP features.6 at B = 512 (8^2 outputs: 128 tall tiles of 4 images)
+    tall = [r for r in fwd if r["block_m"] == 256]
+    assert {r["variant"] for r in tall} == {1281} and {r["block_m"] for r in fwd if r["variant"] == 1281} == {128, 256}
+    for k in (3, 1):
+        assert any(r["stride"] == 2 and r["KH"] == k for r in tall), f"no tall {k}x{k} stride-2 conv"
+    assert any(r["TN"] == 2 for r in tall), "no tall launch with two images per 128-row box"
+    assert any(r["max_per_cta"] > 1 and r["remainder"] != 0 for r in tall), "no tall launch with several tiles per CTA and a remainder"
+    assert any(r["stats"] and r["variant"] % 10 == 1 and r["max_per_cta"] > 1 for r in fwd), "no nsplit-1 epilogue statistics over several tiles per CTA"
+    assert any(r["run"] == "half_eval_folded" and r["bias"] for r in tall), "no folded tall launch with bias"
+    secs = {n: round(RUNS[n][2], 1) for n in runs}
     print("audit wall time per run (s):", secs)
 
 
